@@ -1,14 +1,14 @@
 #!/usr/bin/env python3
 """
-bench.py -- BASELINE.json metric on B200: reads/s (+ GCUPS) of the adapter-alignment hot path.
+bench.py -- BASELINE.json metric on H100: reads/s (+ GCUPS) of the adapter-alignment hot path.
 
 Main line (default --workload endtrim = BASELINE.json configs[1]): 1 M synthetic ~8 kb ONT reads (seed 20260923, SURVEY
 8(d)), adapter set SQK-NSK007 (= the LSK109 Y-adapter), end-trim only: per read the 150-nt start window vs Y_Top (28 nt)
 and the 150-nt end window vs Y_Bottom (22 nt) -> 2 alignments, 7 500 DP cells, 372 algorithmic bytes per read.  A "step"
 is one pass of the hot path over the whole batch.
 
-The same JSON line carries a `configs` block with a reduced-step run of the other BASELINE configs (each with its own
-value / e2e / roofline / parity gate / cpu_baseline):
+The same JSON line carries a `configs` block with a run of the other BASELINE configs, with the same --steps and
+--warmup (each with its own value / e2e / roofline / parity gate / cpu_baseline):
   demux   configs[2]  1 M reads x 356 adapter sequences (all 119 sets + 12 native-full + 96 rapid-full), end windows
   middle  configs[3]  full-read middle-adapter scan, 5 % chimeras: 10 M reads over 8 GPUs = 1.25 M reads per GPU
   sweep   configs[4]  read-length sweep 500 bp - 100 kb x the 192 forward-barcode sequences, 2.5e8 bases per length and GPU
@@ -28,6 +28,9 @@ value / e2e / roofline / parity gate / cpu_baseline):
 
 Launch: python bench.py [--gpus N --steps K --warmup W]; for N>1 via torchrun (one rank per GPU).  --scaling weak
 (default): every rank processes its own full-size batch; --scaling strong: the batch is split over the ranks.
+--dump-outputs DIR: after the timed steps, rank 0 writes the records of the main workload's last device-resident step
+as DIR/<batch>_records.npy (float64, one row of 9 int32 fields per alignment; a fixed seeded sample of rows when all files
+would exceed 64 MB, row indices in DIR/<batch>_rows.npy), so that two builds can be compared output for output.
 """
 import argparse
 import json
@@ -51,7 +54,7 @@ OUT_CAP_BYTES = 320 << 20          # e2e: records copied back per call (larger b
 def parse_args():
     ap = argparse.ArgumentParser()
     ap.add_argument('--gpus', type=int, default=1)
-    ap.add_argument('--steps', type=int, default=10)
+    ap.add_argument('--steps', type=int, default=10, help='timed steps of the main line and of every `configs` entry')
     ap.add_argument('--warmup', type=int, default=3)
     ap.add_argument('--impl', default='b200', choices=['b200', 'reference'])
     ap.add_argument('--workload', default='endtrim', choices=['endtrim', 'demux', 'middle', 'sweep'])
@@ -69,7 +72,37 @@ def parse_args():
                          'device, 4 + 4*adapters bytes per window come back instead of 36 per alignment')
     ap.add_argument('--opt', action='append', default=[], metavar='NAME=VALUE',
                     help='engine option for this run (pb200SetOption), e.g. --opt scratch_mb=72')
+    ap.add_argument('--dump-outputs', default=None, metavar='DIR',
+                    help="write the main workload's records of the last timed step as DIR/<batch>_records.npy")
     return ap.parse_args()
+
+
+DUMP_CAP_BYTES = 64 * 10 ** 6     # everything --dump-outputs writes (below both 64 MB and 64 MiB)
+NPY_HEADER_BYTES = 128
+
+
+def dump_outputs(out_dir, workload, dev):
+    """Records of the last device-resident step, as float64 (exact for every int32 field).  When the files would exceed
+    DUMP_CAP_BYTES, each batch keeps the same share of rows, chosen by a fixed seed, and their indices go to
+    <batch>_rows.npy (float64, 8 more bytes per kept row); an unsampled batch has no _rows.npy."""
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    total_rows = sum(int(d[4].shape[0]) for d in dev)
+    budget = DUMP_CAP_BYTES - 2 * NPY_HEADER_BYTES * len(dev)
+    sampled = total_rows * 9 * 8 > budget
+    cap_rows = budget // (9 * 8 + 8)
+    for (name, _, _, _), d in zip(workload.batches, dev):
+        rec = d[4]
+        n = int(rec.shape[0])
+        rows_path = os.path.join(out_dir, name + '_rows.npy')
+        if sampled:
+            k = max(1, n * cap_rows // total_rows)
+            rows = np.sort(np.random.default_rng(12345).choice(n, size=k, replace=False))
+            rec = rec[torch.from_numpy(rows).to(rec.device)]
+            np.save(rows_path, rows.astype(np.float64))
+        elif os.path.exists(rows_path):
+            os.remove(rows_path)          # left by an earlier sampled run: these records are complete
+        np.save(os.path.join(out_dir, name + '_records.npy'), rec.cpu().numpy().astype(np.float64))
 
 
 # ------------------------------------------------------------------------------------------------------------------
@@ -82,6 +115,7 @@ class ClockSampler(threading.Thread):
         self.samples = []
         self.reasons = set()
         self.sm_max = None
+        self.power_limit_w = None
         self.stop_flag = False
         self.active = False
         self.h = None
@@ -91,8 +125,14 @@ class ClockSampler(threading.Thread):
             self.nv = pynvml
             self.h = pynvml.nvmlDeviceGetHandleByIndex(index)
             self.sm_max = int(pynvml.nvmlDeviceGetMaxClockInfo(self.h, pynvml.NVML_CLOCK_SM))
+            self.power_limit_w = pynvml.nvmlDeviceGetPowerManagementLimit(self.h) / 1000.0
         except Exception:
             self.nv = None
+            try:
+                self.power_limit_w = float(subprocess.check_output(
+                    ['nvidia-smi', '--query-gpu=power.limit', '--format=csv,noheader,nounits', '-i', str(index)], timeout=20))
+            except Exception:
+                pass
 
     def run(self):
         if self.nv is None:
@@ -212,7 +252,7 @@ def make_workload(name, args, rank, world, main, limit=None, alloc=None):
 
 def cgroup_cpu_limit():
     """CPUs the cgroup lets this process use at once (cpu.max = "quota period", v1: cfs_quota_us / cfs_period_us), or None.
-    Round 2: the GPU boxes show nproc = 128 under a quota of 16 CPUs -- threads beyond the quota only get throttled."""
+    A host may show many more hardware threads than its quota lets run; threads beyond the quota only get throttled."""
     try:
         with open('/sys/fs/cgroup/cpu.max') as f:
             q, p = f.read().split()[:2]
@@ -339,7 +379,7 @@ def cpu_baseline(workload, sample_reads=0, sweep=True, seconds=3.0, want_answers
         sec = files.run(cores, 1, answers)
         runs.append({'threads': cores, 'procs': 1, 'seconds': sec})
     if sweep and cores >= 4:
-        over = min(2 * cores, os.cpu_count() or cores)      # under a cgroup quota, 2x the quota was the best mode on the round-2 box
+        over = min(2 * cores, os.cpu_count() or cores)      # under a cgroup quota, oversubscribing it can still be the fastest mode
         for t in sorted({max(1, cores // 2), over} - {cores}):
             runs.append({'threads': t, 'procs': 1, 'seconds': files.run(t)})
     if cores >= 2:
@@ -497,6 +537,8 @@ def measure_gpu(workload, args, ctx, K, Wm, main):
     launches = W.kernel_launches() - l0
     dev_ms = ev0.elapsed_time(ev1)
     W.synchronize()
+    if args.dump_outputs and main and rank == 0:
+        dump_outputs(args.dump_outputs, workload, dev)
     kinds = W.timing_read_kinds(reset=True)
     W.timing_enable(False)
     clocks_value = sampler.take()
@@ -571,12 +613,14 @@ def measure_gpu(workload, args, ctx, K, Wm, main):
     if os.path.exists(peaks_path):
         peak, peak_src = float(json.load(open(peaks_path))['hbm_gbs']), 'measured (MEASURED_PEAKS.json hbm_gbs)'
     else:
-        peak, peak_src = 6650.0, 'fallback (B200_PROFILING.md)'
+        peak, peak_src = 3350.0, 'H100 SXM data sheet (HBM3, 3.35 TB/s), not measured'
+    props = torch.cuda.get_device_properties(torch.cuda.current_device())
+    n_sm, l2_mb = props.multi_processor_count, getattr(props, 'L2_cache_size', 50 << 20) / 1e6
     # dominant DP kernel of the step = the kind with the largest CUDA-event time (events recorded by the library around
     # every DP launch on the launching stream)
     dom = max(kinds, key=lambda k: kinds[k]['ms']) if kinds else None
     roof, alu = None, None
-    sm_mhz = clocks_value.get('sm_mhz') or 1965.0
+    sm_mhz = clocks_value.get('sm_mhz') or clocks_value.get('sm_max_mhz') or 1980.0
     if dom and kinds[dom]['n']:
         kd = kinds[dom]
         per_step_ms = kd['ms'] / K
@@ -613,13 +657,13 @@ def measure_gpu(workload, args, ctx, K, Wm, main):
         cells_kernel = kd.get('cells') or workload.cells * K * (frac_cells if share_cells else 1.0)   # full-sweep kernels: every cell of their share
         cps = cells_kernel / (kd['ms'] / 1e3)
         if sc.get('instr_per_cell'):
-            peak_cells = 148 * 4 * 32 * sm_mhz * 1e6 / sc['instr_per_cell']
+            peak_cells = n_sm * 4 * 32 * sm_mhz * 1e6 / sc['instr_per_cell']
             alu = {'kernel': dom, 'instr_per_cell': sc['instr_per_cell'], 'source': sc.get('source'),
                    'achieved_cells_per_s': cps, 'peak_cells_per_s': peak_cells, 'frac': cps / peak_cells, 'sm_mhz': sm_mhz,
                    'gcups_kernel': cps / 1e9, 'ms_per_step': per_step_ms}
         else:
             alu = {'kernel': dom, 'achieved_cells_per_s': cps, 'gcups_kernel': cps / 1e9, 'sm_mhz': sm_mhz,
-                   'lane_instr_peak_per_s': 148 * 4 * 32 * sm_mhz * 1e6, 'ms_per_step': per_step_ms}
+                   'lane_instr_peak_per_s': n_sm * 4 * 32 * sm_mhz * 1e6, 'ms_per_step': per_step_ms}
     line = {
         'metric': 'reads/sec', 'value': value, 'unit': 'reads/s', 'n_gpus': world, 'steps': K, 'warmup': Wm,
         'ms_per_step': dev_ms / K, 'higher_is_better': True, 'scaling': args.scaling, 'vs_baseline': None,
@@ -627,7 +671,8 @@ def measure_gpu(workload, args, ctx, K, Wm, main):
         'gcups': total_cells * K / (dev_ms / 1e3) / 1e9,
         'config': workload.config(args.scaling),
         'cells_per_read': workload.cells / max(workload.n, 1),
-        'timing': {'l2': 'inputs %.0f MB per step and rank exceed the 126 MB L2' % (in_bytes / 1e6) if in_bytes > 126e6 else
+        'gpu': {'name': props.name, 'sm_count': n_sm, 'l2_mb': l2_mb, 'power_limit_w': sampler.power_limit_w},
+        'timing': {'l2': 'inputs %.0f MB per step and rank exceed the %.0f MB L2' % (in_bytes / 1e6, l2_mb) if in_bytes > l2_mb * 1e6 else
                          'inputs %.0f MB per step' % (in_bytes / 1e6), 'clock': 'CUDA events on the launching stream (value), '
                    'host clock around synchronous C-ABI calls (e2e); max over ranks'},
         'e2e': {'value': e2e_value, 'unit': 'reads/s', 'h2d_bytes_per_step': h2d_bytes, 'd2h_bytes_per_step': out_bytes,
@@ -711,7 +756,7 @@ def run_b200(args):
     cfgs = {}
     for name in others:
         try:
-            sub = one(name, 2 if name != 'demux' else 1, 1, False)
+            sub = one(name, args.steps, args.warmup, False)
         except Exception as e:                      # a failing side config must not lose the headline
             sub = {'error': repr(e)}
         if rank == 0:
@@ -750,7 +795,7 @@ def reference_cli_anchor():
     ref = os.path.join(ROOT, 'baseline', '_ref')
     runner, fq = os.path.join(ref, 'porechop-runner.py'), os.path.join(ref, 'test', 'test_one_adapter_set.fastq')
     if not (os.path.exists(runner) and os.path.exists(fq)):
-        return {'unavailable': 'baseline/_ref not staged (make -C oracle stage, authoring container)'}
+        return {'unavailable': 'baseline/_ref not staged (make -C oracle stage with PORECHOP_REFERENCE set)'}
     with tempfile.TemporaryDirectory() as d:
         out = os.path.join(d, 'out.fastq')
         times = []
@@ -816,7 +861,7 @@ def run_reference(args):
     line['configs'] = {}
     for name in others:
         try:
-            line['configs'][name] = one(name, 2, 1, False)
+            line['configs'][name] = one(name, args.steps, args.warmup, False)
         except Exception as e:
             line['configs'][name] = {'error': repr(e)}
     line['configs']['cli_anchor'] = reference_cli_anchor()

@@ -1,5 +1,5 @@
 /*
- * include/porechop_b200.h -- C-ABI of the B200 adapter-alignment engine (cpp_functions.so).
+ * include/porechop_b200.h -- C-ABI of the H100 adapter-alignment engine (cpp_functions.so).
  *
  * Drop-in boundary (SURVEY.md 8(b)): the library is loaded by ctypes exactly like the reference's
  * porechop/cpp_functions.so (porechop/cpp_function_wrappers.py:21-39) and exports the reference's two
@@ -8,7 +8,7 @@
  *
  * Plain C types only (no torch / CUDA types): pointers, sizes, ints.  Every call runs on the CUDA
  * device that is current for the calling thread (cudaSetDevice / torch.cuda.set_device /
- * pb200SetDevice); there is NO CPU fallback -- without a usable sm_100 device the batch calls return
+ * pb200SetDevice); there is NO CPU fallback -- without a usable sm_90 (H100) device the batch calls return
  * PB200_ERR_NO_DEVICE and adapterAlignment() returns NULL after printing the reason to stderr.
  */
 #ifndef PORECHOP_B200_H
@@ -157,7 +157,7 @@ int pb200TimingReadKinds(double *ms, long long *launches, double *window_cells, 
  *                 memory when every slot is one read x two adapters (cross-product mode); 0 = always computed
  *   "tight_window" 1 (default) = second-pass windows sized per alignment from the end cell's row and score; 0 = the
  *                 per-adapter worst case
- * (round 2 measured and removed "short2p", "rowoff" and the trace-kernel profiles: profiles/r2_options) */
+ * ("short2p", "rowoff" and trace-kernel query profiles were measured and removed: none was faster) */
 int pb200SetOption(const char *name, const char *value);
 /* Current value of an integer tunable ("h2d_pack", "pack_threads", "tight_window", "profile", "scratch_mb", "direct_max",
  * "chunk_tasks", "hbuf" as 0/1/2), or "h2d_pack_large_submit": what h2d_pack = auto resolves to for a large submit on this
@@ -170,7 +170,7 @@ void *pb200HostBuffer(int slot, size_t bytes);
 
 enum {
     PB200_OK = 0,
-    PB200_ERR_NO_DEVICE = 100,   /* no CUDA device / driver, or device is not sm_100 */
+    PB200_ERR_NO_DEVICE = 100,   /* no CUDA device / driver, or device is not sm_90 */
     PB200_ERR_CUDA = 101,        /* a CUDA call failed (see pb200LastError) */
     PB200_ERR_ARG = 102,         /* invalid argument */
     PB200_ERR_INTERNAL = 103     /* internal invariant violated (e.g. window bound) */

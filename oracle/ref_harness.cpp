@@ -9,8 +9,8 @@
 // usage: ref_harness <lib.so> <workload.bin> <threads> [answers.txt]
 //   env REF_HARNESS_PROCS=P (P > 1): P forked worker PROCESSES x <threads> threads each pull chunks from one shared
 //   counter -- every process has its own heap, which separates the machine's capacity from glibc-arena contention
-//   (the reference mallocs an (n+1)(m+1) trace matrix per call; round 1 saw 128 threads in one process run 6x slower on
-//   one host than on another).  Answers are only written in the single-process mode.
+//   (the reference mallocs an (n+1)(m+1) trace matrix per call, so many threads of one process can contend on the
+//   allocator).  Answers are only written in the single-process mode.
 //   workload.bin (little endian), written by porechop_b200.workloads.write_harness_file():
 //     int64 n_seqs, n_adapters, n_pairs ; int32 ma, mi, go, ge ; int32 cross, pad
 //     int64 seq_off[n_seqs+1] ; bytes seqs ; int32 ad_off[n_adapters+1] ; bytes adapters

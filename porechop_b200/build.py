@@ -1,6 +1,6 @@
 """Build cpp_functions.so (the CUDA engine behind the reference's ctypes boundary) in-tree with nvcc.
 
-    python -m porechop_b200.build            # builds porechop_b200/cpp_functions.so for sm_100a
+    python -m porechop_b200.build            # builds porechop_b200/cpp_functions.so for sm_90a (H100)
 
 The file name and location mirror the reference (porechop/cpp_functions.so next to
 cpp_function_wrappers.py, Makefile:24 / cpp_function_wrappers.py:21-25 of the reference).
@@ -41,7 +41,7 @@ def build(force=False, verbose=False):
                         HOSTPACK], capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError('g++ failed on hostpack.cpp:\n' + r.stdout + r.stderr)
-    cmd = [nvcc_path(), '-gencode', 'arch=compute_100a,code=sm_100a', '-O3', '-lineinfo', '-std=c++17',
+    cmd = [nvcc_path(), '-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '-std=c++17',
            '-Xcompiler', '-fPIC', '-shared', '-o', TARGET] + os.environ.get('PB200_NVCC_FLAGS', '').split() + SOURCES + \
           [obj, '-lpthread', '-ldl']
     if verbose:

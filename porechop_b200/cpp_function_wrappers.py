@@ -1,5 +1,5 @@
 """
-ctypes wrapper around cpp_functions.so -- the B200 adapter-alignment engine.
+ctypes wrapper around cpp_functions.so -- the H100 adapter-alignment engine.
 
 Mirror of the reference's porechop/cpp_function_wrappers.py (same module name, same library file name next
 to the module, same `adapter_alignment(read_sequence, adapter_sequence, scoring_scheme_vals) -> str`
@@ -7,7 +7,7 @@ signature and result string, reference lines 21-63), plus the batched call the P
 every (read window, adapter) / (full read, adapter) pair at once (SURVEY.md 8(b)).
 
 There is no CPU fallback: if cpp_functions.so is missing the import exits like the reference does
-(cpp_function_wrappers.py:23-24), and every call raises if no sm_100 CUDA device is usable.
+(cpp_function_wrappers.py:23-24), and every call raises if no sm_90 (H100) CUDA device is usable.
 """
 
 import os

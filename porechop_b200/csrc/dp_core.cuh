@@ -1,9 +1,9 @@
 // porechop_b200/csrc/dp_core.cuh
 //
-// Core of the B200 adapter-alignment engine: the packed-int16 (s16x2, DPX) cell recurrence, the
+// Core of the H100 adapter-alignment engine: the packed-int16 (s16x2, DPX) cell recurrence, the
 // per-lane wavefront step, best-end-cell tracking, traceback and alignment statistics.
 //
-// Semantics follow the reference hot path (paths relative to /root/reference, seqan/ =
+// Semantics follow the reference hot path (paths relative to a Porechop v0.2.4 checkout, seqan/ =
 // porechop/include/seqan/) -- nothing here is ported code, only the arithmetic contract:
 //   cell        seqan/align/dp_formula_affine.h:459-495 ; linear case dp_formula_linear.h:156-188
 //   borders     seqan/align/dp_formula.h:204-220, dp_cell_affine.h:62-64
@@ -88,7 +88,7 @@ PB_HD void unpack_nibbles8(uint32_t w, uint32_t &first4, uint32_t &next4) {
 }
 PB_HD uint32_t unpack_nibble1(uint32_t packed_byte, int odd) { return odd ? (packed_byte & 0xF0u) : ((packed_byte & 0x0Fu) << 4); }
 
-// ---- packed s16x2 primitives (Blackwell DPX: VIADD.16x2 / VIMNMX.S16x2 / VIADDMNMX.S16x2 / VIMNMX3) ----
+// ---- packed s16x2 primitives (DPX instructions of sm_90: __viaddmax_s16x2, __vibmax_s16x2, __vimax3_s16x2) ----
 PB_HD uint32_t add2(uint32_t a, uint32_t b) {
 #if defined(__CUDA_ARCH__)
     return __vadd2(a, b);
@@ -276,8 +276,7 @@ PB_HD void lane_init(Lane<R> &L, int g, int G, const Scoring &sc, const uint8_t 
     L.botX = L.X[R - 1]; L.botV = sc.negb2;
     // candidate (0, m): S = 0, no correction.  Only the bottom row of lane G-1 is the last row: every other lane starts from
     // +infinity, so its compare never fires and the scout branch of the step loops is taken for real candidates only
-    // (round 2, ncu source view: with all 32 lanes tracking their own bottom rows the "rare" branch ran in most steps and
-    // made up 14 % of the trace kernel's dynamic instructions).
+    // (with all 32 lanes tracking their own bottom rows the "rare" branch would run in most steps).
     L.lrBest2 = (g == G - 1) ? sc.borderX2 : 0x7FFF7FFFu;
     L.lrV2 = sc.negb2; L.lrH2 = sc.negb2;
     for (int h = 0; h < 2; ++h) {
@@ -302,10 +301,8 @@ PB_HD uint32_t xnor2(uint32_t a, uint32_t b) {
 // on_alu picks the PIPE of the two accumulations: the flag bits of a step are disjoint, so add / or / xor give the same word,
 // but a predicated add issues on the FMA-heavy pipe (VIADD / IMAD.IADD) and a predicated logic op on the ALU pipe (LOP3).
 // Both pipes take one warp instruction per two cycles and scheduler and the FMA-lite pipe takes no integer work
-// (tools/ubench_pipes.cu under ncu, profiles/r2_pipes: VIMNMX / VIADDMNMX / VIMNMX3 / LOP3 -> ALU; VIADD.16x2 / IMAD /
-// VIADD -> FMA-heavy; alone each sustains 0.5 warp instructions per clock, alternating they reach 1.0).  With every
-// accumulation an add the trace pass had 12 heavy and 6 ALU instructions per row (ncu: fmaheavy 72 %, ALU 57 % busy) and
-// was bound by the heavy pipe; lane_step mixes the two forms (PB_FLAG_ALU_*).
+// (tools/ubench_pipes.cu measures which pipe each instruction issues on).  With every accumulation an add the trace pass
+// has 12 heavy and 6 ALU instructions per row and is bound by the heavy pipe; lane_step mixes the two forms (PB_FLAG_ALU_*).
 // (on_alu is a constant after unrolling: the dead form is eliminated)
 PB_HD uint32_t max2acc(bool on_alu, uint32_t a, uint32_t b, uint32_t &accLo, uint32_t clo, uint32_t &accHi, uint32_t chi) {
 #if defined(__CUDA_ARCH__)
@@ -335,10 +332,8 @@ PB_HD uint32_t max2acc(bool on_alu, uint32_t a, uint32_t b, uint32_t &accLo, uin
 #endif
 }
 // which of a cell's four flag accumulations use the ALU-pipe form: bit 0 tH, 1 tV, 2 tM, 3 tD; _A for even rows of a lane,
-// _B for odd rows.  Measured on B200 (profiles/r2_pipes, end-trim launch of 1 M 150x28 alignments): none 2.083 ms; one of the
-// four (2 of the 8 accumulations per row): tD 1.958, tH 1.976, tH on even rows only 2.037; tH+tV on even rows 1.990, tH+tV
-// 2.053, tH+tV+tM 2.248 -- the minimum is where the hot loop's ALU and FMA-heavy instruction counts are equal (279 / 286 per
-// 4 steps x 7 rows; ncu afterwards: both pipes 69-70 % busy, issue slots 78 %).
+// _B for odd rows.  The default (tD) puts 2 of the 8 accumulations per row on the ALU pipe, which makes the hot loop's ALU
+// and FMA-heavy instruction counts about equal (279 / 286 per 4 steps x 7 rows of the end-trim class).
 #ifndef PB_FLAG_ALU_A
 #define PB_FLAG_ALU_A 0x8
 #endif
@@ -349,8 +344,8 @@ PB_HD uint32_t max2acc(bool on_alu, uint32_t a, uint32_t b, uint32_t &accLo, uin
 // Query profile of the score pass (option "profile", default on).  The substitution operand of group row q depends only
 // on the read base -- six possible codes (0..4 and the read padding code 5).  When both halves of a slot read the same
 // sequence (cross mode: one read, two adapters), score_kernel<.., PROF> keeps those words per lane group in shared memory
-// and fetches a column's R operands with two 128-bit loads instead of computing them with LOP3 + VIADDMNMX per row
-// (measured on B200: 15.8 -> 14.6 ms per launch of the middle scan).  The word is produced by the very expression
+// and fetches a column's R operands with two 128-bit loads instead of computing them with LOP3 + VIADDMNMX per row.
+// The word is produced by the very expression
 // lane_step uses, so both paths are identical by construction.
 // the two base-independent operands of a group row (adapter codes and mismatch operands, as lane_init sets them up) ...
 PB_HD void profile_row(int q, const Scoring &sc, const uint8_t *adA, int mA, int padA, const uint8_t *adB, int mB, int padB,
@@ -372,9 +367,8 @@ PB_HD uint32_t profile_from(uint32_t v2, uint32_t sf2, uint32_t bcode, const Sco
 // negative carries 1 into the high half when added as one 32-bit number (the low half of a biased X is always larger than
 // the addend's magnitude), so that 1 is taken off the high half up front; a non-negative low half never carries (biased
 // values stay below 2^15 + |addend|).  The diagonal term S_diag + sub then is an ordinary integer add (FMA-heavy pipe) --
-// which ptxas cannot fuse into a VIADDMNMX on the ALU pipe, the busier pipe of the score pass (ncu round 2: ALU 65 %,
-// FMA-heavy 22 %) -- and the cell's maximum becomes one three-input VIMNMX3: 3 ALU + 2 heavy instructions per row instead
-// of 4 + 1 (middle scan 28.16 -> 27.89 ms per launch on its own; 107 instead of 115 registers).
+// which ptxas cannot fuse into a VIADDMNMX on the ALU pipe, the busier pipe of the score pass -- and the cell's maximum
+// becomes one three-input VIMNMX3: 3 ALU + 2 heavy instructions per row instead of 4 + 1, and fewer registers.
 PB_HD uint32_t profile_plain(uint32_t sub2) { return (sub2 & 0x8000u) ? sub2 - 0x10000u : sub2; }
 #define PB_PROF_ENCODE(x) profile_plain(x)
 PB_HD uint32_t profile_word(int q, uint32_t bcode, const Scoring &sc, const uint8_t *adA, int mA, int padA, const uint8_t *adB,
@@ -399,11 +393,11 @@ template <int R> PB_HD int trace_shift(int h, int r) { return (R <= 4) ? (4 * r 
 //       bit3 tH : horizontal gap extended  (h_ext >= h_open, ties -> extend)
 //   vr          : KEEPV only -- Vs[j][row] of every owned row (the final-column scout needs it for the end-cell
 //                 correction flags); the hot path does not keep these registers alive
-// Pipe balance of the trace pass (per row, sm_100a; measured in round 2, see max2acc): VIMNMX x4, VIADDMNMX, LOP3 and the
+// Pipe balance of the trace pass (per row, see max2acc): VIMNMX x4, VIADDMNMX, LOP3 and the
 // two xor flag ops run on the ALU pipe (8); the three packed adds (VIADD.16x2), the six predicated flag adds and the X
 // update run on the FMA-heavy pipe (10); the per-step overhead (selects, scout, index arithmetic) is mostly ALU work, which
 // evens the two out over a chunk.  (The gap extension as a plain subtraction instead of the packed add -- both are
-// FMA-heavy work -- measured the same: 2.075 vs 2.083 ms.)
+// FMA-heavy work -- measured the same.)
 #define PB_EXT(x) add2((x), sc.ge2)
 //   PROF / subs : the R substitution operands of this column are given (query profile, see profile_word) instead of being
 //                 computed from h2 -- two ALU-pipe instructions per row less; only when both halves read the same base
@@ -570,7 +564,7 @@ PB_HD int traceback_stats_cur(Cursor &cur, const EndCell &end, bool linear, int 
     }
     // ONE path step per loop iteration with the step kind as data (no per-direction code paths, no inner gap-run loops):
     // the lanes of a warp that trace at the same time run the same instruction stream instead of serialising diagonal /
-    // vertical / horizontal branches and waiting for each other's gap runs (measured on B200: trace launch 2.36 -> 2.25 ms).
+    // vertical / horizontal branches and waiting for each other's gap runs.
     while (j > 0 && i > 0) {
         const bool isD = dir == 0, isV = dir == 1, isH = dir == 2;
         const bool consR = !isV, consA = !isH;              // the step consumes a read base / an adapter base

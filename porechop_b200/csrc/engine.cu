@@ -3,7 +3,7 @@
 // Replaces, behind the same ctypes boundary, the reference's C shim + SeqAn DP + ScoredAlignment
 // (porechop/src/adapter_align.cpp:11-44, porechop/src/alignment.cpp:6-121, seqan/align/dp_*.h).
 // The host side only plans and pipelines: chunking, class selection by adapter length, host<->device
-// copies on a ring of streams, kernel launches.  All alignment arithmetic runs in the sm_100a kernels of
+// copies on a ring of streams, kernel launches.  All alignment arithmetic runs in the sm_90a kernels of
 // kernels.cuh; there is no CPU alignment path in this library.
 #include <cuda_runtime.h>
 
@@ -95,13 +95,13 @@ struct HostBuf {
 };
 
 struct Options {
-    int64_t direct_max = 160;      // longest sequence aligned in a single (trace) pass.  Round 2 on B200: 150-column windows are 6 % faster in one
-                                   // pass, 500-column reads 2.9x faster in two (the one-pass trace of a long window is 10.5 instead of 3.7
-                                   // instructions per cell and its scratch, 129 KB per warp at 500 columns, leaves 2 blocks per SM)
+    int64_t direct_max = 160;      // longest sequence aligned in a single (trace) pass: 150-column end windows are faster in one pass,
+                                   // long reads in two (the one-pass trace of a long window is 10.5 instead of 3.7 instructions per
+                                   // cell and its scratch, 129 KB per warp at 500 columns, leaves 2 blocks per SM)
     int64_t chunk_tasks = 1 << 17; // alignments per pipeline chunk (host-buffer API)
     int64_t device_chunk_tasks = 8 << 20; // alignments per launch group (device-resident API)
     int64_t chunk_bytes = 64ll << 20;   // sequence bytes per pipeline chunk (host-buffer API)
-    int scratch_mb = 128;          // cap on the resident trace scratch (MB); 72 keeps it L2-resident at ~10% lower speed (DESIGN.md)
+    int scratch_mb = 128;          // cap on the resident trace scratch (MB); see launch_trace_variant
     int profile = 1;               // 1: score pass fetches the substitution operands from a shared-memory query profile (same-read slots)
     int tight_window = 1;          // 1: second-pass windows sized per alignment from the end cell's row and score (window_cols)
     int h2d_pack = 0;              // 1: host-buffer API converts to 4-bit codes on the host cores and uploads half the bytes; 0 (default):
@@ -123,8 +123,8 @@ void load_env_options() {
         if (g_opt.pack_threads <= 0) {
             // packer threads: the host's hardware threads shared by the ranks of this node (torchrun exports
             // LOCAL_WORLD_SIZE, and OMP_NUM_THREADS=1 -- which would otherwise leave the packer single-threaded), at most 32
-            // -- and no more than the cgroup CPU quota allows to run at once (round 2: the GPU boxes show 128 hardware threads
-            // under a quota of 16 CPUs; a team larger than the quota is only throttled)
+            // -- and no more than the cgroup CPU quota allows to run at once (a host may show many more hardware
+            // threads than its quota lets run; a team larger than the quota is only throttled)
             unsigned hw = std::max(1u, std::thread::hardware_concurrency());
             if (FILE *f = fopen("/sys/fs/cgroup/cpu.max", "r")) {
                 char q[64]; long long period = 0;
@@ -213,9 +213,9 @@ struct Engine {
         if (init_done) return 0;
         cudaDeviceProp prop;
         CK(cudaGetDeviceProperties(&prop, device));
-        if (prop.major != 10)
+        if (prop.major != 9 || prop.minor != 0)
             return fail(PB200_ERR_NO_DEVICE, "device is sm_" + std::to_string(prop.major * 10 + prop.minor) +
-                                                 ", this library is built for sm_100a only");
+                                                 ", this library is built for sm_90a (H100) only");
         sm_count = prop.multiProcessorCount;
         smem_optin = prop.sharedMemPerBlockOptin;
         for (int i = 0; i < NSTAGE; ++i) CK(cudaStreamCreateWithFlags(&st[i].stream, cudaStreamNonBlocking));
@@ -299,11 +299,11 @@ int launch_trace_variant(Engine &E, Stage &S, cudaStream_t stream, const TaskSrc
     if (int rc = E.blocks_per_sm(reinterpret_cast<const void *>(kern), wpb * 32, smem_bytes, &bps)) return rc;
     const size_t gwarp_bytes = ((size_t)((max_steps + PB_TCHUNK - 1) / PB_TCHUNK) * PB_TCHUNK * WPS * 32 +
                                 (HS ? 0 : (((size_t)SPW * max_n + 31) & ~(size_t)31))) * 4;   // 128-byte lines per warp (kernels.cuh)
-    // The trace scratch of the resident grid is rewritten slot after slot and mostly lives in L2.  `scratch_mb` caps
-    // it (whole blocks per SM, never below 2): measured on B200 for 150x28 windows, 72 MB (3 blocks/SM) keeps the
-    // trace L2-resident (DRAM traffic 1.9x the algorithmic bytes) at ~10 % lower kernel throughput than the default
-    // 128 MB (5 blocks/SM), where ~1.1 GB of dead/dirty trace lines per launch are written back to HBM off the critical
-    // path (8 % of the HBM bandwidth).  See DESIGN.md, "trace scratch".
+    // The trace scratch of the resident grid is rewritten slot after slot and partly lives in L2.  `scratch_mb` caps
+    // it (whole blocks per SM, never below 2).  A smaller cap keeps more of the trace in L2 but leaves fewer warps
+    // resident: on H100 (50 MB L2) 72 MB made the end-trim launches 23 % slower than the default 128 MB, the smallest cap
+    // that reaches the kernel's occupancy limit; the dead trace lines written back to HBM are off the critical path.
+    // See DESIGN.md, "trace scratch".
     int64_t max_blocks = std::max<int64_t>(2 * E.sm_count, (int64_t)(((size_t)g_opt.scratch_mb << 20) / std::max<size_t>(gwarp_bytes * wpb, 1)));
     max_blocks -= max_blocks % E.sm_count;     // whole blocks per SM: the grid-stride loop gives every block the same work
     const int64_t n_tasks = ts.n_tasks;
@@ -718,14 +718,12 @@ int64_t chunk_cap(size_t k, int64_t total_tasks) {
     return std::max<int64_t>(4096, g_opt.chunk_tasks >> (3 - k));
 }
 
-// Packed upload or not for a submit of `total_bytes` of sequence.  Measured on B200 + Xeon 8562Y+ under a 16-CPU quota
-// (round 2, 316 MB per step): the packed path is bound by the host conversion, ~51 GB/s with a 14-thread team = 6.2 ms per
-// step against 6.8 ms for the plain upload (PCIe) and 4.2 ms of kernels; with 8 threads or fewer it is slower than PCIe.  So
-// "auto" packs only large submits and only when the team is large enough (one rank per GPU on a box with few CPUs per rank --
-// e.g. 8 ranks under that quota -- uploads the ASCII bytes as they are).  The gain depends on how many host cycles the
-// process really gets: repeated runs on the same box gave 6.2-6.7 ms packed (once 8.2 ms inside a longer bench run) against
-// a steady 6.8 ms plain, and non-temporal stores in the packer made it slower (7.06 vs 6.66 ms: the DMA engine then reads
-// the codes from DRAM instead of the last-level cache) -- so the default stays the plain upload and packing is an option.
+// Packed upload or not for a submit of `total_bytes` of sequence.  The packed path is bound by the host conversion, so it
+// only pays against the plain PCIe upload with a large packer team; with 8 threads or fewer it is slower.  So "auto" packs
+// only large submits and only when the team is large enough (one rank per GPU on a box with few CPUs per rank uploads the
+// ASCII bytes as they are).  The gain depends on how many host cycles the process really gets, and non-temporal stores in
+// the packer make it slower (the DMA engine then reads the codes from DRAM instead of the last-level cache) -- so the
+// default stays the plain upload and packing is an option.
 bool pack_wanted(int64_t total_bytes) {
     if (total_bytes <= 0 || g_opt.h2d_pack == 0) return false;
     if (g_opt.h2d_pack > 0) return true;
@@ -767,8 +765,8 @@ struct ChunkPlanner {
 
 // Packer: a persistent host thread per engine that plans the chunks of a submit and converts them to 4-bit codes (option
 // h2d_pack; hostpack.cpp, OpenMP team of pack_threads) AHEAD of the submit loop, into a ring of NPACK pinned buffers -- the
-// conversion of chunk k+1.. runs while the submit loop enqueues chunk k and the device works on chunk k-1 (round 2: with
-// the packer inside the submit loop the e2e step was bound by the host conversion, profiles/r2_options).
+// conversion of chunk k+1.. runs while the submit loop enqueues chunk k and the device works on chunk k-1 (with the
+// packer inside the submit loop the e2e step would be bound by the host conversion).
 constexpr int NPACK = NSTAGE + 2;
 struct Packer {
     std::thread th;

@@ -86,7 +86,7 @@ __attribute__((target("avx512f,avx512bw"))) void pack_avx512(const uint8_t *in, 
     int64_t i = i0;
     // the packed bytes are only read back by the DMA engine: non-temporal stores skip the read-for-ownership of the output
     // lines (a third of the loop's memory traffic) when the destination is 32-byte aligned (the engine's pinned buffers are)
-    static const bool want_stream = getenv("PB200_PACK_NT") && atoi(getenv("PB200_PACK_NT")) != 0;   // A/B switch (round 2), default off
+    static const bool want_stream = getenv("PB200_PACK_NT") && atoi(getenv("PB200_PACK_NT")) != 0;   // A/B switch, default off
     const bool stream = want_stream && ((reinterpret_cast<uintptr_t>(out) + (uintptr_t)(i0 >> 1)) & 31) == 0;
     for (; i + 64 <= i1; i += 64) {
         const __m512i x = _mm512_loadu_si512(reinterpret_cast<const void *>(in + i));
@@ -115,9 +115,9 @@ void pack_range(const uint8_t *in, int64_t i0, int64_t i1, int64_t n, uint8_t *o
     pack_scalar(in, i0, i1, n, out);
 }
 
-// A small persistent team for the packer.  Round 2: under OpenMP the team's idle threads spin after every parallel region;
-// the GPU boxes run inside a cgroup CPU quota (16 CPUs under 128 hardware threads), a spinning team eats the quota and the
-// whole process gets throttled (a 64-thread team: 74 ms instead of 6 ms per step).  These workers sleep on a condition
+// A small persistent team for the packer.  Under OpenMP the team's idle threads spin after every parallel region; inside a
+// cgroup CPU quota smaller than the host's hardware threads a spinning team eats the quota and the whole process gets
+// throttled.  These workers sleep on a condition
 // variable between calls and take 64-KB blocks from a shared counter while a call runs.
 class PackTeam {
     std::vector<std::thread> workers;

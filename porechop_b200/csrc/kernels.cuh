@@ -1,4 +1,4 @@
-// porechop_b200/csrc/kernels.cuh -- sm_100a kernels of the adapter-alignment engine.
+// porechop_b200/csrc/kernels.cuh -- sm_90a kernels of the adapter-alignment engine.
 //
 //   encode_kernel        ASCII -> Dna5 code (seqan/basic/alphabet_residue_tabs.h:113-140), HBM-bound
 //   unpack_kernel        host-packed 4-bit codes -> the same code bytes (option h2d_pack)
@@ -231,9 +231,8 @@ __device__ __forceinline__ uint32_t pack_bases(uint32_t bA, uint32_t bB) {
 
 // Stage the packed read bases of a slot's columns: hbuf[c] = pack_bases(A[c], B[c]) for c < nmax, PB_PAD_H past the end
 // of a half.  Each lane of the group builds every G-th column from single-byte streaming loads.
-// (Round 2 A/B on B200, profiles/r2_options: walking the window in 16-column blocks with one aligned 128-bit load per half
-// and block, funnel-shifted into place, was SLOWER -- end-trim launch 2.229 vs 2.180 ms, demux 5.420 vs 5.351 ms: the shift /
-// extract / bounds work per column outweighs the saved LSU instructions (LSU pipe 7 %), so the byte loads stay.)
+// (Walking the window in 16-column blocks with one aligned 128-bit load per half and block, funnel-shifted into place, was
+// slower: the shift / extract / bounds work per column outweighs the saved LSU instructions, so the byte loads stay.)
 template <int G>
 __device__ __forceinline__ void stage_columns(uint32_t *hbuf, int g, const uint8_t *seqA, int nA, const uint8_t *seqB, int nB,
                                               int nmax) {
@@ -250,8 +249,8 @@ __device__ __forceinline__ void stage_columns(uint32_t *hbuf, int g, const uint8
 // Forward wavefront with a 4-bit trace per cell (two 32-bit words per lane per step), then traceback + statistics
 // by two lanes of the group, 9-int record per alignment.  Grid-stride over "warp slots" so the trace scratch is
 // bounded by the resident grid and stays in L2.
-// (Measured and removed in round 2, profiles/r2_options: a score-only first pass + bounded trace window for 150-column
-// windows, and shared-memory query profiles for the substitution operands -- neither beat this single pass on B200.)
+// (Measured and removed: a score-only first pass + bounded trace window for 150-column windows, and shared-memory query
+// profiles for the substitution operands -- neither beat this single pass.)
 template <int G, int R, bool HBUF_SMEM>
 __global__ void __launch_bounds__(PB_WARPS_PER_BLOCK * 32, PB_TRACE_MIN_BLOCKS)
 trace_kernel(const TaskSrc ts, const uint8_t *__restrict__ seq,
@@ -473,9 +472,8 @@ __device__ __forceinline__ uint64_t load_cols(const uint8_t *p) {
 }
 
 // 6 blocks per SM (<= 85 registers: the profile variant compiles to 79-84 without spills; 36 KB of shared memory per block
-// with 16-bit ring entries): the score pass is latency-bound ("wait" 2.6 + shared-memory scoreboard 2.1 stall cycles per
-// issued instruction at 4 warps per scheduler, ncu round 2), so more resident warps pay -- middle scan on B200: 28.16 ms per
-// launch at 4 blocks, 26.27 at 5, 24.28 at 6.  (Fetching the profile operands one step ahead did not: 26.27 / 24.33.)
+// with 16-bit ring entries): the score pass is latency-bound (dependent-chain and shared-memory scoreboard stalls), so more
+// resident warps pay.  (Fetching the profile operands one step ahead did not.)
 #ifndef PB_SCORE_MIN_BLOCKS
 #define PB_SCORE_MIN_BLOCKS 6
 #endif
@@ -488,13 +486,12 @@ __device__ __forceinline__ uint64_t load_cols(const uint8_t *p) {
 // per-group table in shared memory (6 base codes x G*R rows, two 128-bit loads per step) instead of being computed
 // (LOP3 + VIADDMNMX per row): 5 instead of 7 instructions per row, 4 instead of 6 on the ALU pipe -- the pipe that bounds
 // this kernel.  The ring then holds the table offset of a column's base instead of the packed bases.
-// Shared-memory layout (round 2, ncu: the shared-memory data pipe of this kernel was 97 % busy with 2.6x the ideal number of
-// wavefronts -- bank conflicts, not bytes, bounded the score pass):
+// Shared-memory layout (free of bank conflicts -- conflicts, not bytes, bounded an earlier layout of the score pass):
 //   profile table   per group and base code two PLANES of G x 4 words: plane 0 holds the operands of every lane's rows 0..3,
 //                   plane 1 those of rows 4..7, lane g's four words at g*4.  A 128-bit load of 8 consecutive lanes then reads 32
 //                   consecutive words (one wavefront); with G = 4 the two groups of a quarter-warp sit 16 banks apart
-//                   (STRIDE = 16 mod 32).  (Round 1 kept a lane's 8 words together: the first load of 8 lanes touched only
-//                   half the banks, twice.)
+//                   (STRIDE = 16 mod 32).  (Keeping a lane's 8 words together would make the first load of 8 lanes
+//                   touch only half the banks, twice.)
 //   ring            every group's ring is padded to 64 + 2G entries = 32 + G words: all groups of a warp read the same ring index
 //                   in the same instruction, and unpadded rings put that index in the same bank for every group (8-way).
 template <int G, int R> struct ProfGeom {
@@ -542,9 +539,8 @@ score_kernel(const TaskSrc ts, unsigned long long *__restrict__ counter,
 
     // fetch this lane's CPL columns of block `blk` (raw bytes; columns past the end are fixed up when stored).  PROF: both
     // halves read sequence A, only its bytes are fetched.
-    // (Round 2, ncu source view of the middle scan: fetch + store were 4.2 % of the kernel's instructions and 1.4 % of its
-    // stall samples, the loads alone 0.9 % -- the most a TMA bulk copy into the ring could remove, since the byte -> ring
-    // entry conversion and the shared-memory stores stay; not built.  Skipping half B and the per-column bounds tests of
+    // (Fetch + store are a few % of the kernel's instructions, the loads alone less -- the most a TMA bulk copy into the
+    // ring could remove, since the byte -> ring entry conversion and the shared-memory stores stay; not built.  Skipping half B and the per-column bounds tests of
     // interior blocks in the profile variant removes about a third of it.)
     auto fetch = [&](int blk) {
         const int c0 = blk * PB_BLK + g * CPL;
@@ -584,7 +580,7 @@ score_kernel(const TaskSrc ts, unsigned long long *__restrict__ counter,
     for (;;) {
         // every read of the previous segment is ordered before the ring stores below.  (The lanes cannot drift apart anyway --
         // each step's full-mask shuffle joins them, and a block is overwritten 25+ steps after its last read -- but a shuffle
-        // is not a memory barrier: compute-sanitizer racecheck reported the write-after-read pair in round 2.)
+        // is not a memory barrier: compute-sanitizer racecheck reports the write-after-read pair without it.)
         __syncwarp();
         if (!exhausted) {
             if (t >= T) {                      // group-uniform: this group's slot is finished (or none yet)
@@ -650,7 +646,7 @@ score_kernel(const TaskSrc ts, unsigned long long *__restrict__ counter,
                 uint32_t recvS = __shfl_up_sync(0xffffffffu, L.botX, 1, G);
                 uint32_t recvV = __shfl_up_sync(0xffffffffu, L.botV, 1, G);
                 // lane 0 of a group takes the border instead: as a multiply-add (x * 0 + border / x * 1 + 0) the two selects are
-                // FMA-heavy work -- the ALU pipe is the busier one in this kernel (72 % vs 47 % after the bank-conflict fix)
+                // FMA-heavy work -- the ALU pipe is the busier one in this kernel
                 recvS = recvS * top_keep + top_addS;
                 recvV = recvV * top_keep + top_addV;
                 const int j = t - g + 1;

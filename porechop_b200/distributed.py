@@ -68,7 +68,7 @@ def bind_host_to_gpu(pci_bus_id, local_world=1, local_rank=0):
     Pin this process to the CPU cores of the NUMA node its GPU hangs off (sysfs: /sys/bus/pci/devices/<bdf>/numa_node,
     /sys/devices/system/node/nodeK/cpulist), sharing the node's cores between the ranks whose GPUs sit on it.  Pinned
     host buffers allocated afterwards are first-touched on that node, so the rank's H2D / D2H copies and its host-side
-    packing stay NUMA-local (round 1: the e2e step stretched from 7.1 to 8.4 ms at 8 ranks without this).
+    packing stay NUMA-local.
     Returns {'node': k, 'cpus': n} or None when the topology cannot be read (nothing is changed then).
     """
     import os

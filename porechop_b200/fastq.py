@@ -352,8 +352,7 @@ def find_middle_hits(batch, start_trim, end_trim, adapters, middle_threshold, sc
         return hits
     a, b = trimmed_ranges(batch.lengths(), start_trim, end_trim)
     # the trimmed reads of the chunk go into the engine's pinned staging buffer (reused chunk after chunk, uploaded by DMA at
-    # PCIe speed) when there is one -- round 2 on the B200 host: the gather into fresh pageable memory + its upload were most of
-    # the 0.53 s the middle scan of 200 k reads took, the device needing 0.03 s
+    # PCIe speed) when there is one: a gather into fresh pageable memory + its upload would take far longer than the device
     pinned = getattr(W, 'pinned_buffer', None)
     tbuf, toff = _gather_ranges(batch.seq, batch.seq_off[:-1] + a, batch.seq_off[:-1] + b,
                                 alloc=(lambda nbytes: pinned(0, nbytes)) if pinned is not None else None)

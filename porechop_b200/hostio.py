@@ -14,8 +14,8 @@ EXPORTED_SYMBOLS = ['pbioSetThreads', 'pbioCountLines', 'pbioLineEnds', 'pbioLin
 
 
 def usable_cpus():
-    """CPUs this process can really run on at once: the affinity mask capped by the cgroup CPU quota (the GPU boxes of round 2
-    show 128 hardware threads under a quota of 16 CPUs; a larger team only gets the whole process throttled)."""
+    """CPUs this process can really run on at once: the affinity mask capped by the cgroup CPU quota (a host may show many
+    more hardware threads than its quota lets run; a larger team only gets the whole process throttled)."""
     try:
         n = len(os.sched_getaffinity(0))
     except (AttributeError, OSError):

@@ -1,8 +1,8 @@
 #!/usr/bin/env python3
-"""Generate the committed golden fixtures from the UNMODIFIED reference (authoring container only).
+"""Generate the committed golden fixtures from the UNMODIFIED reference (tests/helpers.py REFERENCE).
 
 Runs the reference C++ (oracle/_ref/cpp_functions.so, built by oracle/Makefile from
-/root/reference/porechop/src/*.cpp + vendored SeqAn) through its own C-ABI
+<REFERENCE>/porechop/src/*.cpp + vendored SeqAn) through its own C-ABI
 (porechop/include/adapter_align.h:12-16) and imports the reference's adapter table
 (porechop/adapters.py:77-498) to write:
 
@@ -12,14 +12,17 @@ Runs the reference C++ (oracle/_ref/cpp_functions.so, built by oracle/Makefile f
   tests/golden/golden_windows.json   reference strings for 150-nt end windows x a panel of adapters
   tests/golden/golden_fullread.json  reference strings for full reads (incl. '-'-masked re-alignments)
   tests/golden/golden_random.json    reference strings for seeded random / edge-case inputs
+  tests/golden/golden_live.json      reference strings for the seeded cases of tests/helpers.py live_cases()
 
-/root/reference does not exist on the GPU box, so nothing at test time reads it; only these files.
+Nothing at test time reads the reference checkout; only these files.
 """
 import ctypes, json, os, random, sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
-REF = '/root/reference'
+sys.path.insert(0, os.path.dirname(HERE))
+from helpers import REFERENCE as REF, live_cases  # noqa: E402
+
 sys.path.insert(0, REF)
 
 lib = ctypes.CDLL(os.path.join(ROOT, 'oracle', '_ref', 'cpp_functions.so'))
@@ -157,8 +160,10 @@ def main():
         sc = random.choice(schemes)
         rnd.append([rd, ad, sc, ref_align(rd, ad, sc)])
     json.dump(rnd, open(os.path.join(HERE, 'golden_random.json'), 'w'))
+    live = [ref_align(rd, ad, sc) for rd, ad, sc in live_cases()]
+    json.dump(live, open(os.path.join(HERE, 'golden_live.json'), 'w'), indent=0)
     print('adapters', len(sets), 'full', len(full), 'reads', len(reads), 'windows', len(win), 'fullread', len(fr),
-          'random', len(rnd))
+          'random', len(rnd), 'live', len(live))
 
 
 if __name__ == '__main__':

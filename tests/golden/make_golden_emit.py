@@ -1,6 +1,6 @@
 #!/usr/bin/env python3
 """Golden vectors for the flat FASTQ pipeline (porechop_b200/fastq.py::trim_fastq): whole-CLI outputs of the
-UNMODIFIED reference (porechop.main() imported from /root/reference, running on oracle/_ref/cpp_functions.so) on a
+UNMODIFIED reference (porechop.main() imported from tests/helpers.py REFERENCE, running on oracle/_ref/cpp_functions.so) on a
 small synthetic FASTQ of this repo's own making.  Authoring container only; writes tests/golden/golden_emit.json.
 
 The input is built to hit the corners of the reference's load / trim / split / write code: lower-case bases, an RNA
@@ -21,7 +21,8 @@ import warnings
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
-REF = '/root/reference'
+sys.path.insert(0, os.path.dirname(HERE))
+from helpers import REFERENCE as REF  # noqa: E402  (a Porechop v0.2.4 checkout)
 warnings.simplefilter('ignore')
 
 lib = ctypes.CDLL(os.path.join(ROOT, 'oracle', '_ref', 'cpp_functions.so'))

@@ -1,6 +1,6 @@
 #!/usr/bin/env python3
 """Golden vectors for the batched phase drivers (porechop_b200/phases.py), produced by the UNMODIFIED reference
-Python (porechop/porechop.py + nanopore_read.py + adapters.py imported from /root/reference) running on the
+Python (porechop/porechop.py + nanopore_read.py + adapters.py imported from tests/helpers.py REFERENCE) running on the
 UNMODIFIED reference C++ (oracle/_ref/cpp_functions.so).  Authoring container only; writes
 tests/golden/golden_phases.json.
 
@@ -17,7 +17,8 @@ import warnings
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
-REF = '/root/reference'
+sys.path.insert(0, os.path.dirname(HERE))
+from helpers import REFERENCE as REF  # noqa: E402  (a Porechop v0.2.4 checkout)
 warnings.simplefilter('ignore')
 
 lib = ctypes.CDLL(os.path.join(ROOT, 'oracle', '_ref', 'cpp_functions.so'))

@@ -2,11 +2,15 @@
 import ctypes
 import json
 import os
+import random
 
 import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLDEN = os.path.join(ROOT, 'tests', 'golden')
+# Porechop v0.2.4 checkout the CLI-level comparisons run (its Python package cannot be part of this repository);
+# the same default as oracle/Makefile's.  Tests that need it skip where it does not exist.
+REFERENCE = os.environ.get('PORECHOP_REFERENCE', '/root/reference')
 DEFAULT = [3, -6, -5, -2]
 
 
@@ -98,6 +102,23 @@ def emu_slot(a, b, G, R, mode, sc):
     st = emu_lib().emu_align_slot(a[0].encode(), len(a[0]), a[1].encode(), len(a[1]), (b[0] if b else '').encode(), nb,
                                   (b[1] if b else '').encode(), len(b[1]) if b else 0, G, R, mode, *sc, mx, den, ra, rb)
     return st, list(ra), list(rb)
+
+
+def live_cases():
+    """(read, adapter, scoring) of tests/golden/golden_live.json, regenerated from its seed (the file keeps only the
+    reference's strings): random reads over small alphabets, most with a piece of the adapter inserted."""
+    rng = random.Random(99)
+    schemes = [[3, -6, -5, -2], [3, -6, -2, -2], [2, -3, -2, -5], [1, 0, -1, -1], [4, -5, -3, -3]]
+    out = []
+    for _ in range(1500):
+        al = rng.choice(['AC', 'ACGT', 'ACGTN'])
+        ad = ''.join(rng.choice(al) for _ in range(rng.randint(1, 60)))
+        rd = ''.join(rng.choice(al) for _ in range(rng.randint(1, 300)))
+        if rng.random() < 0.6:
+            p = rng.randint(0, len(rd))
+            rd = rd[:p] + ad[rng.randint(0, len(ad) // 2):] + rd[p:]
+        out.append((rd, ad, rng.choice(schemes)))
+    return out
 
 
 def load_golden(name):

@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""Run the REFERENCE'S OWN unittest suite (/root/reference/test/*.py, 85 CLI-level tests, SURVEY.md section 4) against
+"""Run the REFERENCE'S OWN unittest suite (test/*.py of a Porechop checkout, 85 CLI-level tests, SURVEY.md section 4) against
 
     reference   the unmodified CLI on the reference's own C++                (baseline)
     patch       the unmodified CLI with porechop_b200.patch                  (python -m porechop_b200)
@@ -24,6 +24,8 @@ import tempfile
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 REPO = os.path.dirname(os.path.dirname(HERE))
+sys.path.insert(0, os.path.dirname(HERE))
+from helpers import REFERENCE  # noqa: E402
 
 
 def run_mode(mode, engine, ref, pattern, jobs):
@@ -66,7 +68,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--modes', default='reference,patch,flat')
     ap.add_argument('--engine', default='oracle', choices=['oracle', 'sim', 'cuda'])
-    ap.add_argument('--ref', default='/root/reference')
+    ap.add_argument('--ref', default=REFERENCE)
     ap.add_argument('-k', default='')
     ap.add_argument('--jobs', type=int, default=max(1, (os.cpu_count() or 2) // 2))
     ap.add_argument('--json', default='')

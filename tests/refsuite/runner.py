@@ -1,6 +1,6 @@
 #!/usr/bin/env python3
 """Stand-in for the reference's porechop-runner.py while ITS OWN unittest suite runs (tests/refsuite/run_reference_suite.py
-copies this file next to a copy of /root/reference/test).  TEST INFRASTRUCTURE ONLY.
+copies this file next to a copy of the reference's test/).  TEST INFRASTRUCTURE ONLY.
 
 PB200_SUITE_MODE   reference  the unmodified CLI on the reference's own C++ (oracle/_ref/cpp_functions.so) -- the baseline
                    patch      the unmodified CLI with porechop_b200.patch installed (phases prefetched as batches)

@@ -55,7 +55,7 @@ inline cudaError_t cudaGetDeviceCount(int *n) { *n = 1; return cudaSuccess; }
 inline cudaError_t cudaGetDevice(int *d) { *d = 0; return cudaSuccess; }
 inline cudaError_t cudaSetDevice(int) { return cudaSuccess; }
 inline cudaError_t cudaGetDeviceProperties(cudaDeviceProp *p, int) {
-    p->major = 10; p->minor = 0;
+    p->major = 9; p->minor = 0;
     p->multiProcessorCount = getenv("PBSIM_SMS") ? atoi(getenv("PBSIM_SMS")) : 2;   // small grids: the grid-stride loops really loop
     p->sharedMemPerBlockOptin = 227 * 1024;
     return cudaSuccess;

@@ -1,7 +1,7 @@
 """GPU tier (pytest -m gpu): engine options and the entry points beyond the plain batch call -- packed upload (h2d_pack),
 window bounds (tight_window on / off), query profile of the score pass (profile on / off), global staging (hbuf), the multi
-submit, device decisions, error paths.  No option may change a single record.  (Round 2 measured every opt-in path of
-round 1 on B200 and removed the ones that did not win: profiles/r2_options.)  The file sorts last on purpose."""
+submit, device decisions, error paths.  No option may change a single record.  (Opt-in paths that did not win were
+removed.)  The file sorts last on purpose."""
 import random
 
 import numpy as np

@@ -280,7 +280,7 @@ def test_simulated_engine_results_do_not_depend_on_lane_interleaving():
 
 
 def test_cpu_quota_is_respected_by_the_cpu_baseline_sizing_and_hostio(monkeypatch, tmp_path):
-    """Round 2: the GPU boxes show 128 hardware threads under a cgroup quota of 16 CPUs.  bench.py sizes the CPU baseline and
+    """A host may show many more hardware threads than its cgroup CPU quota lets run.  bench.py sizes the CPU baseline and
     hostio its OpenMP team by what the quota allows, not by the visible threads."""
     import builtins
     import importlib

@@ -1,8 +1,8 @@
-"""CPU tier (authoring container only): the REFERENCE'S OWN unittest suite (/root/reference/test/*.py, 85 CLI-level
+"""CPU tier (needs the Porechop checkout, helpers.REFERENCE): the REFERENCE'S OWN unittest suite (test/*.py, 85 CLI-level
 tests -- SURVEY.md section 4) run against the two drop-ins, with the reference CLI on its own C++ as the baseline
 (tests/refsuite/run_reference_suite.py).  The engine under the drop-ins is the product's own engine.cu + kernels.cuh in the
 host simulation of tests/sim (`--engine sim`; `--engine oracle` uses the C restatement instead, `--engine cuda` the real
-device on a GPU box that has a checkout).
+device).
 
   patch  (python -m porechop_b200)            every one of the 85 tests has the baseline's outcome -- including the three
                                               tests that fail against the reference itself at this commit (SURVEY 0.10)
@@ -14,12 +14,11 @@ import sys
 
 import pytest
 
-from helpers import ROOT
+from helpers import REFERENCE as REF, ROOT
 
-REF = '/root/reference'
 pytestmark = pytest.mark.skipif(not (os.path.isdir(os.path.join(REF, 'test')) and
                                      os.path.exists(os.path.join(ROOT, 'oracle', '_ref', 'cpp_functions.so'))),
-                                reason='needs the reference checkout and oracle/_ref (authoring container)')
+                                reason='needs the Porechop checkout (PORECHOP_REFERENCE) and oracle/_ref built from it')
 
 # tests whose assertions include text of the reference's progress report (adapter table, "N / M reads ...", barcode table)
 REPORT_TESTS = {

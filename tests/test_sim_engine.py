@@ -13,7 +13,7 @@ import sys
 import numpy as np
 import pytest
 
-from helpers import DEFAULT, ROOT, load_golden, oracle_batch
+from helpers import DEFAULT, REFERENCE, ROOT, load_golden, oracle_batch
 from test_oracle import SURVEY_EDGE, rebuild_fullread_inputs
 
 sys.path.insert(0, os.path.join(ROOT, 'tests', 'sim'))
@@ -263,7 +263,7 @@ def test_sim_end_decisions_and_flat_pipeline(W, monkeypatch):
 
 
 # ---- the GPU tier's own test functions, run on the simulated engine -------------------------------------------------
-# (same code, same sizes as on the B200; excluded: tests that need torch CUDA tensors, 10^6-read properties and threads)
+# (same code, same sizes as on the GPU; excluded: tests that need torch CUDA tensors, 10^6-read properties and threads)
 GPU_PARITY = ['test_legacy_single_call_strings', 'test_golden_random_pair_list', 'test_golden_windows_cross',
               'test_golden_fullread_two_pass', 'test_synthetic_windows_vs_oracle', 'test_demux_cross_all_adapters_vs_oracle',
               'test_ragged_and_edge_inputs', 'test_long_reads_two_pass_vs_oracle', 'test_read_length_sweep_barcodes',
@@ -335,7 +335,7 @@ def _sim_as_engine(W):
     return install
 
 
-@pytest.mark.skipif(not os.path.isdir('/root/reference/porechop'), reason='needs the reference checkout (authoring container)')
+@pytest.mark.skipif(not os.path.isdir(os.path.join(REFERENCE, 'porechop')), reason='needs the Porechop checkout (PORECHOP_REFERENCE)')
 def test_sim_engine_under_the_unmodified_cli_and_the_flat_cli(W, monkeypatch, tmp_path):
     """tests/test_patch_cli.py and tests/test_flat_cli.py compare the drop-ins with the reference CLI byte for byte, with the
     oracle standing in for the engine; here the same comparisons run on the product's engine code (host simulation): the

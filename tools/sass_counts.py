@@ -3,7 +3,7 @@
 
     python tools/sass_counts.py profiles/<round>_trace_kernel.ncu-rep profiles/<round>_score_kernel.ncu-rep ...
 
-Input: `ncu --set full --import-source on` reports of bench.py launches (tools/gpu_call.sh, stage ncu).  For every kernel in a
+Input: `ncu --set full --import-source on` reports of bench.py launches.  For every kernel in a
 report the SASS page gives, per instruction, how often it was executed.  The hot loop is the set of instructions that share
 the most frequent execution count weighted by its size (the unrolled straight-line step loop: every one of its instructions
 runs exactly once per iteration, nothing else in the kernel runs that often AND is that large).  With `steps` wavefront steps
@@ -74,6 +74,7 @@ def main():
     for fam, pick in (('trace_kernel', 'trace_kernel<4,7>'), ('score_kernel', 'score_kernel<4,8>')):
         if pick in res:
             res[fam] = dict(res[pick])
+    os.makedirs(os.path.join(ROOT, 'profiles'), exist_ok=True)      # git-ignored: measured output, per GPU
     p = os.path.join(ROOT, 'profiles', 'sass_counts.json')
     json.dump(res, open(p, 'w'), indent=1, sort_keys=True)
     for k, v in sorted(res.items()):

@@ -1,11 +1,11 @@
-// tools/ubench_pipes.cu -- which PIPE the instructions of the DP kernels issue on, and at what rate (sm_100a).
+// tools/ubench_pipes.cu -- which PIPE the instructions of the DP kernels issue on, and at what rate (sm_90a).
 // Each kernel runs 8 independent chains per thread of one op (or two ops alternating), 8 warps per scheduler.  Printed:
 // warp-instructions per clock and scheduler from clock64; run under
 //   ncu --metrics smsp__inst_executed.sum,smsp__issue_active.avg.pct_of_peak_sustained_active,\
 //       sm__pipe_alu_cycles_active.avg.pct_of_peak_sustained_active,sm__pipe_fmaheavy_cycles_active.avg.pct_of_peak_sustained_active,\
 //       sm__pipe_fmalite_cycles_active.avg.pct_of_peak_sustained_active,sm__pipe_fma_cycles_active.avg.pct_of_peak_sustained_active
-// the pipe counters of every kernel say where its instructions went (round 2: profiles/r2_pipes).
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o ubench_pipes tools/ubench_pipes.cu ; run on the GPU box.
+// the pipe counters of every kernel say where its instructions went.
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o ubench_pipes tools/ubench_pipes.cu ; run on an H100.
 #include <cuda_runtime.h>
 #include <cstdint>
 #include <cstdio>
@@ -73,8 +73,10 @@ __global__ void __launch_bounds__(512) k(uint32_t *out, uint32_t seed, long long
 
 template <int OP> void run(const char *name, int per_chain_instr) {
     uint32_t *out; long long *cyc, h;
-    cudaMalloc(&out, 148 * 1024 * 4 * 4); cudaMalloc(&cyc, 8);
-    for (int rep = 0; rep < 2; ++rep) { k<OP><<<148 * 2, 512>>>(out, 12345u, cyc); cudaDeviceSynchronize(); }   // 32 warps / SM
+    int sms = 0;
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
+    cudaMalloc(&out, (size_t)sms * 2 * 512 * 4); cudaMalloc(&cyc, 8);
+    for (int rep = 0; rep < 2; ++rep) { k<OP><<<sms * 2, 512>>>(out, 12345u, cyc); cudaDeviceSynchronize(); }   // 32 warps / SM
     cudaMemcpy(&h, cyc, 8, cudaMemcpyDeviceToHost);
     const double warp_instr = 8.0 * ITER * 8 * per_chain_instr;   // per scheduler: 8 warps x ITER x 8 chains
     printf("%-44s %.3f warp-instr/clk/scheduler\n", name, warp_instr / h);
