@@ -116,6 +116,35 @@ int adapterAlignmentBatchDevice(const uint8_t *d_seqs, const int64_t *d_seq_off,
                                 const int32_t *ad_off, int32_t n_adapters, int matchScore, int mismatchScore,
                                 int gapOpenScore, int gapExtensionScore, int32_t *d_out, void *stream);
 
+/* Phase C of Porechop on the device: find_middle_adapters (porechop/nanopore_read.py:216-243) for every sequence.
+ * Sequences are the end-trimmed reads; adapters are in the reference's order (porechop.py:541-548).  For each sequence,
+ * for each adapter in order: align; if float("%f" % fullAdapter%ID) >= middle_threshold, record the hit, overwrite read
+ * positions [readStart, readEnd] with the N code (the reference's '-') and align the same adapter again; otherwise move on
+ * to the next adapter.  The masked reads and the records of reads without a hit never leave the device.
+ * Output (caller-owned host buffers): n_hits[s] = number of hits of sequence s; hits = hits_cap records of 10 int32
+ * {adapter index, the 9-int record of the alignment that hit}, sequence-major, each sequence's hits in the order found.
+ * *n_total is always written.  If *n_total > hits_cap, only n_hits and *n_total are valid and the call returns
+ * PB200_ERR_SPACE.
+ * Preconditions, checked before the device is touched (PB200_ERR_ARG otherwise): middle_threshold > 0 (not NaN), every
+ * adapter byte in ACGTUacgtu, and every adapter served by the int16 kernels with a finite window bound (both gap scores
+ * negative).  Under them every hit masks at least one base that was not masked before, so the loop ends; more rounds
+ * than the longest sequence has bases give PB200_ERR_INTERNAL. */
+int adapterMiddleScan(const uint8_t *seqs, const int64_t *seq_off, int64_t n_seqs, const uint8_t *adapters,
+                      const int32_t *ad_off, int32_t n_adapters, int matchScore, int mismatchScore, int gapOpenScore,
+                      int gapExtensionScore, double middle_threshold, int32_t *n_hits, int32_t *hits, int64_t hits_cap,
+                      int64_t *n_total);
+/* Same, with seqs / seq_off in device memory (conventions of adapterAlignmentBatchDevice; the caller's sequences are not
+ * modified: the masking works on the library's encoded copy).  The work is enqueued on `stream`; the outputs are host
+ * buffers, so the call returns only after they are written. */
+int adapterMiddleScanDevice(const uint8_t *d_seqs, const int64_t *d_seq_off, int64_t n_seqs, int64_t total_seq_bytes,
+                            int64_t max_seq_len, const uint8_t *adapters, const int32_t *ad_off, int32_t n_adapters,
+                            int matchScore, int mismatchScore, int gapOpenScore, int gapExtensionScore,
+                            double middle_threshold, int32_t *n_hits, int32_t *hits, int64_t hits_cap, int64_t *n_total,
+                            void *stream);
+/* cmin[l], l = 0 .. len-1: the smallest c with float("%f" % (100.0*c/l)) >= middle_threshold, or l+1 if none does
+ * (cmin[0] = INT32_MAX).  The ">=" sibling of pb200TrimThresholdTable.  Pure host code; middle_threshold must be > 0. */
+int pb200MiddleThresholdTable(double middle_threshold, int32_t len, int32_t *cmin);
+
 /* Format one 9-int record as the reference string (alignment.cpp:113-121). Returns strlen, or -1 if buflen is
  * too small (64 bytes always suffice). */
 int pb200FormatRecord(const int32_t *record, char *buf, int buflen);
@@ -173,7 +202,8 @@ enum {
     PB200_ERR_NO_DEVICE = 100,   /* no CUDA device / driver, or device is not sm_90 */
     PB200_ERR_CUDA = 101,        /* a CUDA call failed (see pb200LastError) */
     PB200_ERR_ARG = 102,         /* invalid argument */
-    PB200_ERR_INTERNAL = 103     /* internal invariant violated (e.g. window bound) */
+    PB200_ERR_INTERNAL = 103,    /* internal invariant violated (e.g. window bound) */
+    PB200_ERR_SPACE = 104        /* an output buffer is too small (adapterMiddleScan: *n_total > hits_cap) */
 };
 
 #ifdef __cplusplus

@@ -12,7 +12,7 @@ There is no CPU fallback: if cpp_functions.so is missing the import exits like t
 
 import os
 import sys
-from ctypes import CDLL, POINTER, Structure, c_char_p, c_double, c_int, c_int32, c_int64, c_longlong, c_void_p, cast, \
+from ctypes import CDLL, POINTER, Structure, byref, c_char_p, c_double, c_int, c_int32, c_int64, c_longlong, c_void_p, cast, \
     create_string_buffer
 
 import numpy as np
@@ -62,6 +62,14 @@ C_LIB.adapterAlignmentBatchMulti.restype = c_int
 C_LIB.adapterAlignmentBatchDevice.argtypes = [c_void_p, c_void_p, c_int64, c_int64, c_int64, c_void_p, c_void_p,
                                               c_int32, c_int, c_int, c_int, c_int, c_void_p, c_void_p]
 C_LIB.adapterAlignmentBatchDevice.restype = c_int
+C_LIB.adapterMiddleScan.argtypes = [c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_int32, c_int, c_int, c_int, c_int,
+                                    c_double, c_void_p, c_void_p, c_int64, c_void_p]
+C_LIB.adapterMiddleScan.restype = c_int
+C_LIB.adapterMiddleScanDevice.argtypes = [c_void_p, c_void_p, c_int64, c_int64, c_int64, c_void_p, c_void_p, c_int32, c_int,
+                                          c_int, c_int, c_int, c_double, c_void_p, c_void_p, c_int64, c_void_p, c_void_p]
+C_LIB.adapterMiddleScanDevice.restype = c_int
+C_LIB.pb200MiddleThresholdTable.argtypes = [c_double, c_int32, c_void_p]
+C_LIB.pb200MiddleThresholdTable.restype = c_int
 C_LIB.pb200FormatRecord.argtypes = [c_void_p, c_char_p, c_int]
 C_LIB.pb200FormatRecord.restype = c_int
 C_LIB.pb200DeviceCount.restype = c_int
@@ -82,22 +90,27 @@ C_LIB.pb200PackNibbles.argtypes = [c_void_p, c_int64, c_void_p, c_int]
 C_LIB.pb200PackNibbles.restype = c_int
 
 EXPORTED_SYMBOLS = ['adapterAlignment', 'freeCString', 'adapterAlignmentBatch', 'adapterAlignmentBatchMulti',
-                    'adapterAlignmentBatchDevice', 'adapterEndDecisions', 'pb200TrimThresholdTable',
+                    'adapterAlignmentBatchDevice', 'adapterEndDecisions', 'pb200TrimThresholdTable', 'adapterMiddleScan',
+                    'adapterMiddleScanDevice', 'pb200MiddleThresholdTable',
                     'pb200FormatRecord', 'pb200DeviceCount', 'pb200SetDevice', 'pb200Synchronize', 'pb200LastError',
                     'pb200KernelLaunches', 'pb200TimingEnable', 'pb200TimingRead', 'pb200TimingReadKinds', 'pb200SetOption',
                     'pb200GetOption', 'pb200HostBuffer', 'pb200PackNibbles']
 
 RECORD_INTS = 9
+HIT_INTS = 10                 # adapterMiddleScan: {adapter index, 9-int record}
 SCORE_EMPTY = -2147483648
+ERR_ARG, ERR_SPACE = 102, 104
 
 
 class EngineError(RuntimeError):
-    pass
+    code = None               # the PB200_ERR_* code of a failed engine call
 
 
 def _check(rc):
     if rc != 0:
-        raise EngineError('porechop_b200 engine error %d: %s' % (rc, C_LIB.pb200LastError().decode()))
+        e = EngineError('porechop_b200 engine error %d: %s' % (rc, C_LIB.pb200LastError().decode()))
+        e.code = rc
+        raise e
 
 
 def adapter_alignment(read_sequence, adapter_sequence, scoring_scheme_vals):
@@ -257,6 +270,62 @@ def adapter_alignment_batch_device(d_seqs_ptr, d_seq_off_ptr, n_seqs, total_seq_
     _check(C_LIB.adapterAlignmentBatchDevice(c_void_p(d_seqs_ptr), c_void_p(d_seq_off_ptr), n_seqs, total_seq_bytes,
                                              max_seq_len, _ptr(ad_buf), _ptr(ad_off), len(ad_off) - 1, ma, mi, go, ge,
                                              c_void_p(d_out_ptr), c_void_p(stream_ptr)))
+
+
+def _middle_scan(call, n_seqs):
+    """adapterMiddleScan(Device) with caller-owned outputs: starts with room for 2n + 1024 hits and retries once with exactly
+    *n_total when the engine answers PB200_ERR_SPACE."""
+    n_hits = np.zeros(n_seqs, dtype=np.int32)
+    total = c_int64(0)
+    cap = 2 * n_seqs + 1024
+    for _ in range(2):
+        hits = np.empty((cap, HIT_INTS), dtype=np.int32)
+        rc = call(_ptr(n_hits), _ptr(hits), cap, byref(total))
+        if rc == ERR_SPACE and total.value > cap:
+            cap = total.value
+            continue
+        _check(rc)
+        return n_hits, hits[:total.value]
+    _check(rc)
+
+
+def adapter_middle_scan(seq_buf, seq_off, ad_buf, ad_off, scoring_scheme_vals, middle_threshold):
+    """
+    Porechop's Phase C on the device (adapterMiddleScan): every hit of every sequence, masking rounds included.
+    seq_buf / seq_off: the end-trimmed reads (uint8, int64[n+1]); ad_buf / ad_off: the adapters in the reference's order.
+    Returns (n_hits int32[n], hits int32[total, 10]): hits are sequence-major, each sequence's in the order found, each
+    {adapter index, 9-int record} -- hits[:, 1:] goes to scores_from_records / format_record as it is.
+    """
+    seq_buf = np.ascontiguousarray(seq_buf, dtype=np.uint8)
+    seq_off = np.ascontiguousarray(seq_off, dtype=np.int64)
+    ad_buf = np.ascontiguousarray(ad_buf, dtype=np.uint8)
+    ad_off = np.ascontiguousarray(ad_off, dtype=np.int32)
+    n_seqs, n_ad = len(seq_off) - 1, len(ad_off) - 1
+    ma, mi, go, ge = [int(x) for x in scoring_scheme_vals]
+    return _middle_scan(lambda nh, h, cap, total: C_LIB.adapterMiddleScan(
+        _ptr(seq_buf), _ptr(seq_off), n_seqs, _ptr(ad_buf), _ptr(ad_off), n_ad, ma, mi, go, ge, float(middle_threshold), nh, h,
+        cap, total), n_seqs)
+
+
+def adapter_middle_scan_device(d_seqs_ptr, d_seq_off_ptr, n_seqs, total_seq_bytes, max_seq_len, ad_buf, ad_off,
+                               scoring_scheme_vals, middle_threshold, stream_ptr=0):
+    """adapter_middle_scan with the reads already in device memory (raw device pointers as ints, the conventions of
+    adapter_alignment_batch_device).  The caller's device buffers are not modified."""
+    ad_buf = np.ascontiguousarray(ad_buf, dtype=np.uint8)
+    ad_off = np.ascontiguousarray(ad_off, dtype=np.int32)
+    ma, mi, go, ge = [int(x) for x in scoring_scheme_vals]
+    return _middle_scan(lambda nh, h, cap, total: C_LIB.adapterMiddleScanDevice(
+        c_void_p(d_seqs_ptr), c_void_p(d_seq_off_ptr), n_seqs, total_seq_bytes, max_seq_len, _ptr(ad_buf), _ptr(ad_off),
+        len(ad_off) - 1, ma, mi, go, ge, float(middle_threshold), nh, h, cap, total, c_void_p(stream_ptr)), int(n_seqs))
+
+
+def middle_threshold_table(middle_threshold, length):
+    """cmin[l] of pb200MiddleThresholdTable: smallest match count whose float("%f") identity reaches middle_threshold."""
+    t = np.zeros(length, dtype=np.int32)
+    rc = C_LIB.pb200MiddleThresholdTable(float(middle_threshold), int(length), _ptr(t))
+    if rc != 0:
+        raise EngineError('pb200MiddleThresholdTable: error %d' % rc)
+    return t
 
 
 def synchronize():

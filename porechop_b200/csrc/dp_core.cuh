@@ -652,6 +652,16 @@ PB_HD int32_t end_trim_candidate(const int32_t *r, int is_start, int32_t end_siz
     if (is_start) return (re == end_size) ? 0 : re + extra_trim;
     return (rs == 0) ? 0 : (end_size - rs) + extra_trim;
 }
+// ---- middle-adapter hits on the device ----------------------------------------------------------------------------
+// find_middle_adapters (porechop/nanopore_read.py:216-243) for one record: float("%f" % (100.0*match_ad/len_ad)) >=
+// middle_threshold, with cmin[len_ad] the smallest passing match count (engine.cu pb200MiddleThresholdTable).  A failed
+// alignment has len_ad = 0 and never hits (cmin[0] is huge, and the threshold is > 0).  The table covers the window bound
+// W(m_max) + 2; a length outside it sets *overflow.
+PB_HD bool middle_hit(const int32_t *r, const int32_t *cmin, int32_t cmin_len, int *overflow) {
+    const int32_t l = r[8], c = r[7];
+    if (l < 0 || l >= cmin_len) { *overflow = 1; return false; }
+    return l > 0 && c >= cmin[l];
+}
 // barcode score column of a record: (match_ad, len_ad) as two uint16 -- the host turns the pair into the exact double
 // the reference parses (full-adapter identity); a failed alignment scores 0.0 = the pair (0, 1).
 PB_HD uint32_t score_pair(const int32_t *r, int *overflow) {

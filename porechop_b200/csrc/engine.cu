@@ -21,6 +21,7 @@
 #include <mutex>
 #include <string>
 #include <thread>
+#include <tuple>
 #include <vector>
 
 #include "../../include/porechop_b200.h"
@@ -187,6 +188,9 @@ struct Engine {
     long long timed_n_acc[TK_N] = {0, 0, 0, 0};
     int next_trace_kind = TK_TRACE;      // set to TK_TRACE_WINDOW around the second-pass launch of a two-pass class
     DevBuf wcells;                       // device counter: DP cells of the windowed second passes (window_tasks_kernel)
+    // middle-adapter scan (adapterMiddleScan*): the resident segment -- codes (masked in place), offsets, records, next adapter
+    // per read, hit slots, two active lists, threshold table, append counter + longest appended read
+    DevBuf mid_codes, mid_off, mid_rec, mid_next_ad, mid_hits, mid_active[2], mid_cmin, mid_ctr;
     std::shared_ptr<void> packer;        // Packer (below): the thread that plans and packs chunks ahead of the submit loop
     // launch constants, queried once per (kernel, dynamic shared-memory size); all users hold `mu`.  The opt-in shared-memory
     // limit is a property of the KERNEL, not of a launch: it is only ever raised (a launch with less is always valid).
@@ -584,15 +588,18 @@ int run_generic_cross(Engine &E, Stage &S, cudaStream_t stream, const ClassPlan 
 
 // Cross product of sequences [s0, s0+cnt) (already encoded on the device, offsets on the device) with all adapters.
 // d_seq_off points at the offset of sequence s0 (cnt+1 entries), base_off is subtracted from every offset.
+// seq_order (optional): slot i is sequence seq_order[i] of d_seq_off (the active reads of a middle-scan round); without it
+// the two-pass path orders the sequences longest first itself.
 int run_cross_chunk(Engine &E, Stage &S, cudaStream_t stream, const AdapterPlan &P, const uint8_t *seq_codes,
                     const int64_t *d_seq_off, int64_t cnt, int64_t base_off, int64_t max_n, int32_t n_adapters,
-                    int32_t *d_out, const int64_t *h_seq_off_abs, int64_t s0, const int32_t *h_ad_off) {
+                    int32_t *d_out, const int64_t *h_seq_off_abs, int64_t s0, const int32_t *h_ad_off,
+                    const int32_t *seq_order = nullptr) {
     if (int rc = S.misc.ensure(64)) return rc;
     int *status = S.misc.as<int>();
     unsigned long long *counter = reinterpret_cast<unsigned long long *>(S.misc.as<char>() + 16);
     // long reads (two-pass path): process sequences longest first
-    const int32_t *d_order = nullptr;
-    if (P.si.bounded && max_n > g_opt.direct_max && cnt > 1) {
+    const int32_t *d_order = seq_order;
+    if (!seq_order && P.si.bounded && max_n > g_opt.direct_max && cnt > 1) {
         if (int rc = S.order.ensure((size_t)cnt * 4)) return rc;
         if (int rc = S.bins.ensure((size_t)PB_ORDER_BINS * 4)) return rc;
         CK(cudaMemsetAsync(S.bins.p, 0, (size_t)PB_ORDER_BINS * 4, stream));
@@ -647,6 +654,42 @@ __global__ void rebase_kernel(int64_t *off, int64_t n, int64_t base) {
 __global__ void stride_offsets_kernel(int64_t *off, int64_t n, int64_t stride) {
     int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) off[i] = i * stride;
+}
+
+// ... and the offsets of a middle-scan chunk, shifted to the segment's resident code buffer (the last entry is also the next
+// chunk's first: both chunks write the same value)
+__global__ void shift_offsets_kernel(const int64_t *in, int64_t *out, int64_t n, int64_t delta) {
+    int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) out[i] = in[i] + delta;
+}
+
+// Resident state of one segment of a middle-adapter scan: the segment's codes (masked in place round after round), offsets of
+// its reads into `codes` (segment-relative read ids), records (read-major), next adapter per read, hit slots, active lists.
+struct MiddleSeg {
+    uint8_t *codes = nullptr;
+    int64_t *off = nullptr;               // off[s], s = 0 .. n (host API: written chunk by chunk in round 0)
+    int64_t n = 0, max_len = 0;
+    int32_t *rec = nullptr, *next_ad = nullptr, *hits = nullptr, *active[2] = {nullptr, nullptr};
+    unsigned *count = nullptr;
+    unsigned long long *max_len_d = nullptr;
+    const int32_t *cmin = nullptr;
+    int32_t cmin_len = 0;
+};
+
+int launch_middle_decide(Engine &E, cudaStream_t stream, const MiddleSeg &M, int32_t n_adapters, const int32_t *active,
+                         int64_t first, int64_t n, int32_t *next_active, int *status) {
+    if (n <= 0) return 0;
+    MiddleArgs a;
+    a.records = M.rec; a.n_adapters = n_adapters;
+    a.active = active; a.first = first; a.n = n;
+    a.next_ad = M.next_ad; a.seq_off = M.off; a.codes = M.codes;
+    a.cmin = M.cmin; a.cmin_len = M.cmin_len;
+    a.hits = M.hits; a.next_active = next_active; a.count = M.count; a.max_len = M.max_len_d;
+    const int64_t blocks = std::min<int64_t>((n + 3) / 4, (int64_t)E.sm_count * 16);
+    middle_decide_kernel<<<(unsigned)blocks, 128, 0, stream>>>(a, status);
+    g_launches++;
+    CK(cudaGetLastError());
+    return 0;
 }
 
 // One pipeline chunk of the host-buffer API: sequences [s0, s1), longest sequence max_n.
@@ -709,6 +752,9 @@ struct CrossJob {
     const int32_t *d_cmin = nullptr; int32_t cmin_len = 0;
     const int32_t *d_cols = nullptr;
     int64_t max_seq_len = 0;          // decision jobs: longest window the threshold table covers
+    // middle scan (adapterMiddleScan): codes, offsets and records go to the segment's resident buffers instead of the stage's,
+    // and middle_decide_kernel runs round 0 on each chunk; nothing is copied back
+    const MiddleSeg *mid = nullptr;
 };
 
 // The first chunks of a submit ramp up (1/8, 1/4, 1/2 of chunk_tasks): the pipeline's fill -- pack + H2D of chunk 0 before
@@ -887,9 +933,11 @@ int run_cross_jobs(Engine &E, std::vector<CrossJob> &jobs, int ma, int mi, int g
             CK(cudaStreamSynchronize(stream));   // previous use of this stage's buffers is complete
         }
         if (int rc = S.seq_raw.ensure((size_t)bytes + 16)) return rc;
-        if (int rc = S.seq_codes.ensure((size_t)bytes + 16)) return rc;
+        if (!J.mid) {
+            if (int rc = S.seq_codes.ensure((size_t)bytes + 16)) return rc;
+            if (int rc = S.out.ensure((size_t)cnt * J.n_adapters * PB_REC * 4)) return rc;
+        }
         if (int rc = S.seq_off.ensure((size_t)(cnt + 1) * 8)) return rc;
-        if (int rc = S.out.ensure((size_t)cnt * J.n_adapters * PB_REC * 4)) return rc;
         {
         NvtxRange r("pb200:h2d");
         if (it.buf >= 0) {
@@ -904,16 +952,28 @@ int run_cross_jobs(Engine &E, std::vector<CrossJob> &jobs, int ma, int mi, int g
         if (!c.uniform) CK(cudaMemcpyAsync(S.seq_off.p, J.seq_off + s0, (size_t)(cnt + 1) * 8, cudaMemcpyHostToDevice, stream));
         }
         NvtxRange dp_range("pb200:dp");
+        const int64_t mid_rel = J.mid ? base - J.seq_off[0] : 0;     // the chunk's first byte in the segment's resident codes
+        uint8_t *codes = J.mid ? J.mid->codes + mid_rel : S.seq_codes.as<uint8_t>();
+        int32_t *recs = J.mid ? J.mid->rec + (size_t)s0 * J.n_adapters * PB_REC : S.out.as<int32_t>();
         if (c.uniform) stride_offsets_kernel<<<(unsigned)((cnt + 1 + 255) / 256), 256, 0, stream>>>(S.seq_off.as<int64_t>(), cnt + 1, c.max_n);
         else rebase_kernel<<<(unsigned)((cnt + 1 + 255) / 256), 256, 0, stream>>>(S.seq_off.as<int64_t>(), cnt + 1, base);
         g_launches++;
-        if (it.buf >= 0) {
-            if (int rc = launch_unpack(stream, S.seq_raw.as<uint8_t>(), S.seq_codes.as<uint8_t>(), bytes, E.sm_count)) return rc;
-        } else {
-            if (int rc = launch_encode(stream, S.seq_raw.as<uint8_t>(), S.seq_codes.as<uint8_t>(), bytes, E.sm_count)) return rc;
+        if (J.mid) {
+            shift_offsets_kernel<<<(unsigned)((cnt + 1 + 255) / 256), 256, 0, stream>>>(S.seq_off.as<int64_t>(), J.mid->off + s0,
+                                                                                     cnt + 1, mid_rel);
+            g_launches++;
         }
-        if (int rc = run_cross_chunk(E, S, stream, P, S.seq_codes.as<uint8_t>(), S.seq_off.as<int64_t>(), cnt, base, c.max_n,
-                                     J.n_adapters, S.out.as<int32_t>(), J.seq_off, s0, J.ad_off)) return rc;
+        if (it.buf >= 0) {
+            if (int rc = launch_unpack(stream, S.seq_raw.as<uint8_t>(), codes, bytes, E.sm_count)) return rc;
+        } else {
+            if (int rc = launch_encode(stream, S.seq_raw.as<uint8_t>(), codes, bytes, E.sm_count)) return rc;
+        }
+        if (int rc = run_cross_chunk(E, S, stream, P, codes, S.seq_off.as<int64_t>(), cnt, base, c.max_n,
+                                     J.n_adapters, recs, J.seq_off, s0, J.ad_off)) return rc;
+        if (J.mid) {
+            if (int rc = launch_middle_decide(E, stream, *J.mid, J.n_adapters, nullptr, s0, cnt, J.mid->active[0],
+                                              S.misc.as<int>())) return rc;
+        }
         if (J.dec) {
             const pb200_end_batch_t &D = *J.dec;
             if (int rc = S.dec_trim.ensure((size_t)cnt * 4)) return rc;
@@ -1159,29 +1219,31 @@ double percent_exact(int32_t c, int32_t l) {
     snprintf(buf, sizeof buf, "%f", 100.0 * cd / ld);
     return strtod(buf, nullptr);
 }
-void trim_threshold_table(double thr, int32_t len, int32_t *cmin) {
+// inclusive = false: the end-trim test (value > thr); true: the middle-hit test (value >= thr)
+void threshold_table(double thr, int32_t len, bool inclusive, int32_t *cmin) {
     if (len > 0) cmin[0] = INT32_MAX;
     for (int32_t l = 1; l < len; ++l) {
-        // percent_exact(., l) is non-decreasing: binary search for the first c with value > thr
+        // percent_exact(., l) is non-decreasing: binary search for the first c that passes
         int32_t lo = 0, hi = l + 1;
         while (lo < hi) {
             const int32_t mid = lo + (hi - lo) / 2;
-            if (percent_exact(mid, l) > thr) hi = mid; else lo = mid + 1;
+            const double v = percent_exact(mid, l);
+            if (inclusive ? v >= thr : v > thr) hi = mid; else lo = mid + 1;
         }
         cmin[l] = lo;
     }
 }
 
-// threshold tables are pure functions of (threshold, length): built once, reused by every later call
-std::shared_ptr<const std::vector<int32_t>> cached_threshold_table(double thr, int32_t len) {
+// threshold tables are pure functions of (threshold, length, test): built once, reused by every later call
+std::shared_ptr<const std::vector<int32_t>> cached_threshold_table(double thr, int32_t len, bool inclusive = false) {
     static std::mutex mu;
-    static std::map<std::pair<double, int32_t>, std::shared_ptr<const std::vector<int32_t>>> cache;
+    static std::map<std::tuple<double, int32_t, bool>, std::shared_ptr<const std::vector<int32_t>>> cache;
     std::lock_guard<std::mutex> lk(mu);
-    const auto key = std::make_pair(thr, len);
+    const auto key = std::make_tuple(thr, len, inclusive);
     auto it = cache.find(key);
     if (it != cache.end()) return it->second;
     auto t = std::make_shared<std::vector<int32_t>>((size_t)len);
-    trim_threshold_table(thr, len, t->data());
+    threshold_table(thr, len, inclusive, t->data());
     if (cache.size() >= 64) cache.clear();                     // growth guard (thresholds are few in practice)
     cache[key] = t;
     return t;
@@ -1246,6 +1308,21 @@ int batch_end_decisions(const pb200_end_batch_t *batches, int n_batches, int ma,
     return run_cross_jobs(E, jobs, ma, mi, go, ge);
 }
 
+// longest sequence of a device-resident batch (S.misc must hold 64 bytes)
+int device_max_len(Stage &S, cudaStream_t stream, const int64_t *d_seq_off, int64_t n_seqs, int64_t *max_len) {
+    unsigned long long *d_max = reinterpret_cast<unsigned long long *>(S.misc.as<char>() + 32);
+    CK(cudaMemsetAsync(d_max, 0, 8, stream));
+    int64_t blocks = std::min<int64_t>((n_seqs + 255) / 256, 1024);
+    max_len_kernel<<<(unsigned)blocks, 256, 0, stream>>>(d_seq_off, n_seqs, d_max);
+    g_launches++;
+    CK(cudaGetLastError());
+    unsigned long long h = 0;
+    CK(cudaMemcpyAsync(&h, d_max, 8, cudaMemcpyDeviceToHost, stream));
+    CK(cudaStreamSynchronize(stream));
+    *max_len = (int64_t)h;
+    return 0;
+}
+
 int batch_device(const uint8_t *d_seqs, const int64_t *d_seq_off, int64_t n_seqs, int64_t total_seq_bytes,
                  int64_t max_seq_len, const uint8_t *adapters, const int32_t *ad_off, int32_t n_adapters, int ma, int mi,
                  int go, int ge, int32_t *d_out, void *user_stream) {
@@ -1267,15 +1344,7 @@ int batch_device(const uint8_t *d_seqs, const int64_t *d_seq_off, int64_t n_seqs
     if (int rc = S.misc.ensure(64)) return rc;
     CK(cudaMemsetAsync(S.misc.as<char>() + 16, 0, 48, stream));   // status word (offset 0) is sticky until pb200Synchronize
     if (max_seq_len < 0) {
-        unsigned long long *d_max = reinterpret_cast<unsigned long long *>(S.misc.as<char>() + 32);
-        CK(cudaMemsetAsync(d_max, 0, 8, stream));
-        int64_t blocks = std::min<int64_t>((n_seqs + 255) / 256, 1024);
-        max_len_kernel<<<(unsigned)blocks, 256, 0, stream>>>(d_seq_off, n_seqs, d_max);
-        g_launches++;
-        unsigned long long h = 0;
-        CK(cudaMemcpyAsync(&h, d_max, 8, cudaMemcpyDeviceToHost, stream));
-        CK(cudaStreamSynchronize(stream));
-        max_seq_len = (int64_t)h;
+        if (int rc = device_max_len(S, stream, d_seq_off, n_seqs, &max_seq_len)) return rc;
     }
     if (max_seq_len > 0x7fff0000ll) return fail(PB200_ERR_ARG, "sequence longer than 2^31");
     std::vector<int64_t> h_off;   // only fetched when a generic class exists
@@ -1293,6 +1362,285 @@ int batch_device(const uint8_t *d_seqs, const int64_t *d_seq_off, int64_t n_seqs
                                      h_off.empty() ? nullptr : h_off.data(), s0, ad_off)) return rc;
     }
     return 0;
+}
+
+
+// ---- middle-adapter scan (adapterMiddleScan, Phase C) ------------------------------------------------------------
+// Host-side checks that make the device loop exact and finite (include/porechop_b200.h): threshold > 0, adapters of A/C/G/T/U
+// only, every adapter in an int16 class with a finite window bound.  cmin_len = W(m_max) + 2 covers every len_ad a traced
+// path (score >= 0) can have.
+int middle_preconditions(const uint8_t *adapters, const int32_t *ad_off, int32_t n_adapters, int ma, int mi, int go, int ge,
+                         double thr, int32_t *cmin_len) {
+    if (!(thr > 0.0)) return fail(PB200_ERR_ARG, "middle_threshold must be > 0 for the device middle scan");
+    const SchemeInfo si = scheme_info(ma, mi, go, ge);
+    if (!si.bounded) return fail(PB200_ERR_ARG, "the device middle scan needs negative gap scores (a finite window bound)");
+    int64_t m_max = 0;
+    for (int32_t a = 0; a < n_adapters; ++a) {
+        const int32_t m = ad_off[a + 1] - ad_off[a];
+        if (class_of(si, m) == GENERIC_CLASS) return fail(PB200_ERR_ARG, "adapter or scheme outside the int16 kernels");
+        for (int32_t k = ad_off[a]; k < ad_off[a + 1]; ++k)
+            if (!strchr("ACGTUacgtu", adapters[k]) || adapters[k] == 0)
+                return fail(PB200_ERR_ARG, "the device middle scan takes adapters of A/C/G/T/U only");
+        m_max = std::max<int64_t>(m_max, m);
+    }
+    *cmin_len = (int32_t)(m_max + (m_max * si.wnum) / si.wden + 2);
+    return 0;
+}
+
+// the hits of one round of one segment, as they came back: read (segment-relative) and {adapter, record} per append position
+struct MiddleRound { int64_t s0; std::vector<int32_t> reads, hits; };
+
+size_t device_free_bytes() {
+#if defined(__CUDACC__)
+    size_t f = 0, t = 0;
+    if (cudaMemGetInfo(&f, &t) != cudaSuccess) { cudaGetLastError(); return 1ull << 30; }
+    return f;
+#else
+    return 4ull << 30;     // host builds of these sources have no device-memory query
+#endif
+}
+
+// The reads [a, b) of the next segment: its resident buffers take at most half of the free device memory (plus what the
+// engine already holds for them) and n * n_adapters stays below 2^31 (records are indexed with int32 out_idx).
+// h_seq_off: host offsets when the segment's codes are part of its resident buffers (host API), else nullptr.
+int64_t middle_segment_end(const Engine &E, int64_t a, int64_t n_seqs, int32_t n_adapters, const int64_t *h_seq_off) {
+    const size_t held = E.mid_codes.cap + E.mid_off.cap + E.mid_rec.cap + E.mid_next_ad.cap + E.mid_hits.cap +
+                        E.mid_active[0].cap + E.mid_active[1].cap;
+    const double budget = (double)(device_free_bytes() + held) / 2;
+    // per read: offset, records, next adapter, hit slot, two active-list entries, the two-pass task and end-cell records
+    const double per_read = 8 + (double)n_adapters * (PB_REC * 4 + sizeof(Task) + 16) + 4 + PB_HIT_INTS * 4 + 8;
+    const int64_t max_reads = std::max<int64_t>(1, std::min<int64_t>(0x7fffffffll / std::max<int32_t>(n_adapters, 1),
+                                                                     (int64_t)(budget / per_read)));
+    int64_t b = std::min(n_seqs, a + max_reads);
+    if (h_seq_off)
+        while (b > a + 1 && (double)(h_seq_off[b] - h_seq_off[a]) + (double)(b - a) * per_read > budget) b = a + (b - a) / 2;
+    return b;
+}
+
+int middle_segment_buffers(Engine &E, int64_t n, int32_t n_adapters, size_t code_bytes, MiddleSeg &M) {
+    if (code_bytes) {
+        if (int rc = E.mid_codes.ensure(code_bytes + 16)) return rc;
+        M.codes = E.mid_codes.as<uint8_t>();
+    }
+    if (int rc = E.mid_off.ensure((size_t)(n + 1) * 8)) return rc;
+    if (int rc = E.mid_rec.ensure((size_t)n * n_adapters * PB_REC * 4)) return rc;
+    if (int rc = E.mid_next_ad.ensure((size_t)n * 4)) return rc;
+    if (int rc = E.mid_hits.ensure((size_t)n * PB_HIT_INTS * 4)) return rc;
+    if (int rc = E.mid_active[0].ensure((size_t)n * 4)) return rc;
+    if (int rc = E.mid_active[1].ensure((size_t)n * 4)) return rc;
+    if (int rc = E.mid_ctr.ensure(64)) return rc;
+    M.n = n;
+    M.rec = E.mid_rec.as<int32_t>(); M.next_ad = E.mid_next_ad.as<int32_t>(); M.hits = E.mid_hits.as<int32_t>();
+    M.active[0] = E.mid_active[0].as<int32_t>(); M.active[1] = E.mid_active[1].as<int32_t>();
+    M.count = E.mid_ctr.as<unsigned>();
+    M.max_len_d = reinterpret_cast<unsigned long long *>(E.mid_ctr.as<char>() + 8);
+    M.cmin = E.mid_cmin.as<int32_t>();
+    return 0;
+}
+
+// Rounds >= 1 of a segment whose round 0 (DP over every read + middle_decide_kernel) has been enqueued on `stream` (or has
+// completed on other streams): each round reads back its hit count and longest active read, copies the round's hits home,
+// and runs the DP over the active reads only (slot i = read active[i]: records land in each read's own slots, nothing is
+// copied or re-encoded) followed by the next middle_decide_kernel.
+int middle_rounds(Engine &E, Stage &S, cudaStream_t stream, const AdapterPlan &P, MiddleSeg &M, int32_t n_adapters,
+                  const int32_t *h_ad_off, int64_t s0, std::vector<MiddleRound> &out) {
+    int cur = 0;                      // round 0 appended to active[0]
+    for (int64_t round = 1;; ++round) {
+        unsigned c = 0;
+        unsigned long long mx = 0;
+        CK(cudaMemcpyAsync(&c, M.count, 4, cudaMemcpyDeviceToHost, stream));
+        CK(cudaMemcpyAsync(&mx, M.max_len_d, 8, cudaMemcpyDeviceToHost, stream));
+        if (int rc = check_status(S, stream)) return rc;
+        if (c == 0) return 0;
+        out.push_back(MiddleRound{s0, std::vector<int32_t>(c), std::vector<int32_t>((size_t)c * PB_HIT_INTS)});
+        CK(cudaMemcpyAsync(out.back().reads.data(), M.active[cur], (size_t)c * 4, cudaMemcpyDeviceToHost, stream));
+        CK(cudaMemcpyAsync(out.back().hits.data(), M.hits, (size_t)c * PB_HIT_INTS * 4, cudaMemcpyDeviceToHost, stream));
+        // every hit masks at least one base that was not masked before (include/porechop_b200.h): a read has at most
+        // max_len hits, so more rounds than that mean a broken invariant, not a long input
+        if (round > M.max_len) return fail(PB200_ERR_INTERNAL, "middle scan: more rounds than the longest sequence has bases");
+        CK(cudaMemsetAsync(E.mid_ctr.p, 0, 16, stream));
+        if (int rc = run_cross_chunk(E, S, stream, P, M.codes, M.off, (int64_t)c, 0, (int64_t)mx, n_adapters, M.rec, nullptr, 0,
+                                     h_ad_off, M.active[cur])) return rc;
+        if (int rc = launch_middle_decide(E, stream, M, n_adapters, M.active[cur], 0, (int64_t)c, M.active[cur ^ 1],
+                                          S.misc.as<int>())) return rc;
+        cur ^= 1;
+    }
+}
+
+// hits of every round of every segment -> n_hits / hits, sequence-major, each sequence's hits in round order
+int middle_emit(const std::vector<MiddleRound> &rounds, int64_t n_seqs, int32_t *n_hits, int32_t *hits, int64_t hits_cap,
+                int64_t *n_total) {
+    memset(n_hits, 0, (size_t)n_seqs * 4);
+    int64_t total = 0;
+    for (const MiddleRound &R : rounds) {
+        for (int32_t s : R.reads) n_hits[R.s0 + s]++;
+        total += (int64_t)R.reads.size();
+    }
+    *n_total = total;
+    if (total > hits_cap) return fail(PB200_ERR_SPACE, "hits_cap is smaller than the number of hits (*n_total)");
+    std::vector<int64_t> at((size_t)n_seqs + 1, 0);
+    for (int64_t s = 0; s < n_seqs; ++s) at[s + 1] = at[s] + n_hits[s];
+    for (const MiddleRound &R : rounds)
+        for (size_t p = 0; p < R.reads.size(); ++p)
+            memcpy(hits + (size_t)(at[R.s0 + R.reads[p]]++) * PB_HIT_INTS, R.hits.data() + p * PB_HIT_INTS, PB_HIT_INTS * 4);
+    return 0;
+}
+
+int middle_table(Engine &E, cudaStream_t stream, double thr, int32_t cmin_len) {
+    const auto table = cached_threshold_table(thr, cmin_len, true);
+    if (int rc = E.mid_cmin.ensure((size_t)cmin_len * 4)) return rc;
+    CK(cudaMemcpyAsync(E.mid_cmin.p, table->data(), (size_t)cmin_len * 4, cudaMemcpyHostToDevice, stream));
+    CK(cudaStreamSynchronize(stream));
+    return 0;
+}
+
+int middle_check_outputs(int64_t n_seqs, int32_t n_adapters, const int32_t *n_hits, const int32_t *hits, int64_t hits_cap,
+                         const int64_t *n_total) {
+    if (n_seqs < 0 || n_adapters < 0 || hits_cap < 0) return fail(PB200_ERR_ARG, "negative count");
+    if (!n_total || (n_seqs > 0 && !n_hits) || (hits_cap > 0 && !hits)) return fail(PB200_ERR_ARG, "NULL pointer");
+    return 0;
+}
+
+int middle_host(const uint8_t *seqs, const int64_t *seq_off, int64_t n_seqs, const uint8_t *adapters, const int32_t *ad_off,
+                int32_t n_adapters, int ma, int mi, int go, int ge, double thr, int32_t *n_hits, int32_t *hits,
+                int64_t hits_cap, int64_t *n_total) {
+    if (int rc = middle_check_outputs(n_seqs, n_adapters, n_hits, hits, hits_cap, n_total)) return rc;
+    if (n_seqs > 0 && (!seq_off || (n_adapters > 0 && !ad_off))) return fail(PB200_ERR_ARG, "NULL pointer");
+    load_env_options();
+    int32_t cmin_len = 0;
+    if (n_adapters > 0) {
+        if (int rc = validate_args(seqs, seq_off, n_seqs, adapters, ad_off, n_adapters, nullptr, nullptr, 0, true)) return rc;
+        if (int rc = middle_preconditions(adapters, ad_off, n_adapters, ma, mi, go, ge, thr, &cmin_len)) return rc;
+    } else if (!(thr > 0.0)) {
+        return fail(PB200_ERR_ARG, "middle_threshold must be > 0 for the device middle scan");
+    }
+    if (n_seqs == 0 || n_adapters == 0) {
+        if (n_seqs > 0) memset(n_hits, 0, (size_t)n_seqs * 4);
+        *n_total = 0;
+        return 0;
+    }
+    int64_t max_len = 0;
+    for (int64_t s = 0; s < n_seqs; ++s) {
+        const int64_t len = seq_off[s + 1] - seq_off[s];
+        if (len < 0) return fail(PB200_ERR_ARG, "sequence offsets not monotone");
+        max_len = std::max(max_len, len);
+    }
+    if (max_len > 0x7fff0000ll) return fail(PB200_ERR_ARG, "sequence longer than 2^31");
+    Engine *Ep = nullptr;
+    if (int rc = get_engine(&Ep)) return rc;
+    Engine &E = *Ep;
+    std::lock_guard<std::mutex> lk(E.mu);
+    if (int rc = E.init()) return rc;
+    NvtxRange submit_range("pb200:submit_middle");
+    Stage &S = E.st[0];
+    cudaStream_t stream = S.stream;
+    std::vector<MiddleRound> rounds;
+    auto run = [&]() -> int {
+        if (int rc = middle_table(E, stream, thr, cmin_len)) return rc;
+        for (int64_t a = 0; a < n_seqs;) {
+            const int64_t b = middle_segment_end(E, a, n_seqs, n_adapters, seq_off);
+            MiddleSeg M;
+            if (int rc = middle_segment_buffers(E, b - a, n_adapters, (size_t)(seq_off[b] - seq_off[a]), M)) return rc;
+            M.off = E.mid_off.as<int64_t>();
+            M.cmin_len = cmin_len;
+            M.max_len = max_len;
+            CK(cudaMemsetAsync(E.mid_ctr.p, 0, 16, stream));
+            CK(cudaStreamSynchronize(stream));
+            // round 0: the chunk pipeline of every other host-buffer call, into the segment's resident buffers
+            std::vector<CrossJob> jobs(1);
+            jobs[0] = CrossJob{seqs, seq_off + a, b - a, adapters, ad_off, n_adapters, nullptr};
+            jobs[0].mid = &M;
+            if (int rc = run_cross_jobs(E, jobs, ma, mi, go, ge)) return rc;
+            AdapterPlan P;
+            if (int rc = plan_adapters(E, stream, adapters, ad_off, n_adapters, ma, mi, go, ge, P)) return rc;
+            if (int rc = middle_rounds(E, S, stream, P, M, n_adapters, ad_off, a, rounds)) return rc;
+            a = b;
+        }
+        return 0;
+    };
+    if (int rc = run()) {                 // nothing may still be running when we return
+        const std::string first_err = g_err;
+        cudaStreamSynchronize(stream);
+        g_err = first_err;
+        return rc;
+    }
+    return middle_emit(rounds, n_seqs, n_hits, hits, hits_cap, n_total);
+}
+
+int middle_device(const uint8_t *d_seqs, const int64_t *d_seq_off, int64_t n_seqs, int64_t total_seq_bytes,
+                  int64_t max_seq_len, const uint8_t *adapters, const int32_t *ad_off, int32_t n_adapters, int ma, int mi,
+                  int go, int ge, double thr, int32_t *n_hits, int32_t *hits, int64_t hits_cap, int64_t *n_total,
+                  void *user_stream) {
+    if (int rc = middle_check_outputs(n_seqs, n_adapters, n_hits, hits, hits_cap, n_total)) return rc;
+    if (total_seq_bytes < 0) return fail(PB200_ERR_ARG, "negative count");
+    if (n_seqs > 0 && (!d_seq_off || (n_adapters > 0 && !ad_off))) return fail(PB200_ERR_ARG, "NULL pointer");
+    load_env_options();
+    int32_t cmin_len = 0;
+    if (n_adapters > 0) {
+        if (int rc = validate_args(nullptr, nullptr, 0, adapters, ad_off, n_adapters, nullptr, nullptr, 0, true)) return rc;
+        if (int rc = middle_preconditions(adapters, ad_off, n_adapters, ma, mi, go, ge, thr, &cmin_len)) return rc;
+    } else if (!(thr > 0.0)) {
+        return fail(PB200_ERR_ARG, "middle_threshold must be > 0 for the device middle scan");
+    }
+    if (n_seqs == 0 || n_adapters == 0) {
+        if (n_seqs > 0) memset(n_hits, 0, (size_t)n_seqs * 4);
+        *n_total = 0;
+        return 0;
+    }
+    Engine *Ep = nullptr;
+    if (int rc = get_engine(&Ep)) return rc;
+    Engine &E = *Ep;
+    std::lock_guard<std::mutex> lk(E.mu);
+    if (int rc = E.init()) return rc;
+    NvtxRange submit_range("pb200:submit_middle");
+    Stage &S = E.st[0];
+    cudaStream_t stream = user_stream ? (cudaStream_t)user_stream : S.stream;
+    std::vector<MiddleRound> rounds;
+    auto run = [&]() -> int {
+        if (!S.misc.p) {
+            if (int rc = S.misc.ensure(64)) return rc;
+            CK(cudaMemsetAsync(S.misc.p, 0, 64, stream));
+        }
+        if (int rc = check_status(S, stream)) return rc;     // a deferred error of an earlier device-resident call
+        AdapterPlan P;
+        if (int rc = plan_adapters(E, stream, adapters, ad_off, n_adapters, ma, mi, go, ge, P)) return rc;
+        if (max_seq_len < 0) {
+            if (int rc = device_max_len(S, stream, d_seq_off, n_seqs, &max_seq_len)) return rc;
+        }
+        if (max_seq_len > 0x7fff0000ll) return fail(PB200_ERR_ARG, "sequence longer than 2^31");
+        if (int rc = middle_table(E, stream, thr, cmin_len)) return rc;
+        // the library's encoded copy of the caller's sequences is what the rounds mask
+        if (int rc = E.mid_codes.ensure((size_t)total_seq_bytes + 16)) return rc;
+        if (int rc = launch_encode(stream, d_seqs, E.mid_codes.as<uint8_t>(), total_seq_bytes, E.sm_count)) return rc;
+        for (int64_t a = 0; a < n_seqs;) {
+            const int64_t b = middle_segment_end(E, a, n_seqs, n_adapters, nullptr);
+            MiddleSeg M;
+            if (int rc = middle_segment_buffers(E, b - a, n_adapters, 0, M)) return rc;
+            M.codes = E.mid_codes.as<uint8_t>();
+            M.off = const_cast<int64_t *>(d_seq_off + a);          // read only: offsets are written by the host-buffer path only
+            M.cmin_len = cmin_len;
+            M.max_len = max_seq_len;
+            CK(cudaMemsetAsync(E.mid_ctr.p, 0, 16, stream));
+            const int64_t max_cnt = std::max<int64_t>(1, g_opt.device_chunk_tasks / n_adapters);
+            for (int64_t c0 = 0; c0 < b - a; c0 += max_cnt) {           // round 0: every read, from adapter 0
+                const int64_t cnt = std::min(max_cnt, b - a - c0);
+                if (int rc = run_cross_chunk(E, S, stream, P, M.codes, M.off + c0, cnt, 0, max_seq_len, n_adapters,
+                                             M.rec + (size_t)c0 * n_adapters * PB_REC, nullptr, 0, ad_off)) return rc;
+                if (int rc = launch_middle_decide(E, stream, M, n_adapters, nullptr, c0, cnt, M.active[0], S.misc.as<int>()))
+                    return rc;
+            }
+            if (int rc = middle_rounds(E, S, stream, P, M, n_adapters, ad_off, a, rounds)) return rc;
+            a = b;
+        }
+        return 0;
+    };
+    if (int rc = run()) {
+        const std::string first_err = g_err;
+        cudaStreamSynchronize(stream);
+        g_err = first_err;
+        return rc;
+    }
+    return middle_emit(rounds, n_seqs, n_hits, hits, hits_cap, n_total);
 }
 
 }  // namespace
@@ -1319,7 +1667,30 @@ int adapterEndDecisions(const pb200_end_batch_t *batches, int n_batches, int ma,
 
 int pb200TrimThresholdTable(double end_threshold, int32_t len, int32_t *cmin) {
     if (len < 0 || (len > 0 && !cmin) || !(end_threshold >= 0.0)) return PB200_ERR_ARG;
-    trim_threshold_table(end_threshold, len, cmin);
+    threshold_table(end_threshold, len, false, cmin);
+    return 0;
+}
+
+int adapterMiddleScan(const uint8_t *seqs, const int64_t *seq_off, int64_t n_seqs, const uint8_t *adapters,
+                      const int32_t *ad_off, int32_t n_adapters, int ma, int mi, int go, int ge, double middle_threshold,
+                      int32_t *n_hits, int32_t *hits, int64_t hits_cap, int64_t *n_total) {
+    g_err.clear();
+    return middle_host(seqs, seq_off, n_seqs, adapters, ad_off, n_adapters, ma, mi, go, ge, middle_threshold, n_hits, hits,
+                       hits_cap, n_total);
+}
+
+int adapterMiddleScanDevice(const uint8_t *d_seqs, const int64_t *d_seq_off, int64_t n_seqs, int64_t total_seq_bytes,
+                            int64_t max_seq_len, const uint8_t *adapters, const int32_t *ad_off, int32_t n_adapters, int ma,
+                            int mi, int go, int ge, double middle_threshold, int32_t *n_hits, int32_t *hits, int64_t hits_cap,
+                            int64_t *n_total, void *stream) {
+    g_err.clear();
+    return middle_device(d_seqs, d_seq_off, n_seqs, total_seq_bytes, max_seq_len, adapters, ad_off, n_adapters, ma, mi, go, ge,
+                         middle_threshold, n_hits, hits, hits_cap, n_total, stream);
+}
+
+int pb200MiddleThresholdTable(double middle_threshold, int32_t len, int32_t *cmin) {
+    if (len < 0 || (len > 0 && !cmin) || !(middle_threshold > 0.0)) return PB200_ERR_ARG;
+    threshold_table(middle_threshold, len, true, cmin);
     return 0;
 }
 

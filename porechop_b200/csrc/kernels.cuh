@@ -7,6 +7,7 @@
 //   score_kernel<G,R,P>  streaming score-only overlap DP with exact scout (long reads), dynamic slot refill
 //   window_tasks_kernel  end cells of the score pass -> bounded-window tasks for trace_kernel
 //   decide_kernel        records -> per-read end-trim amounts + barcode score pairs (decisions stay on the device)
+//   middle_decide_kernel one round of the middle-adapter scan: first hit per active read, masking, next active list
 //   generic_kernel       int32 thread-serial fallback for scoring schemes / adapters outside the int16 domain
 //
 // The arithmetic is in dp_core.cuh (shared with the CPU emulation used by the tests).
@@ -767,6 +768,67 @@ __global__ void decide_kernel(const DecideArgs a, int *__restrict__ status) {
                 }
             }
         }
+    }
+    if (ovf) atomicOr(status, 2);
+}
+
+// ---------------------------------------------------------------------------------------------------
+// middle_decide_kernel: one round of find_middle_adapters (porechop/nanopore_read.py:216-243) over the active reads of a
+// resident segment.  One warp per read: the first adapter from the read's current one onward whose record hits
+// (middle_hit) is the round's hit; the warp masks read positions [rs, re] with the N code in the resident code buffer
+// (the byte encode_kernel writes for the reference's '-'), keeps the adapter as the read's next one and appends the read
+// to the next round's active list.  A read without a hit leaves the active set.  Reads own disjoint byte ranges, so the
+// masking needs no synchronisation between warps.  The append position varies from run to run; the hit is written at
+// that position together with the read id (next_active), and the host orders the hits by (read, round), so the result
+// does not depend on it.  Round 0: active == nullptr, the reads are first .. first+n-1 and every read starts at adapter 0.
+struct MiddleArgs {
+    const int32_t *records; int32_t n_adapters;   // segment-wide, read-major: read s's records start at s * n_adapters
+    const int32_t *active; int64_t first, n;      // this round's reads (segment-relative ids), or nullptr (round 0)
+    int32_t *next_ad;                             // per read: the adapter its next round starts from
+    const int64_t *seq_off; uint8_t *codes;       // resident offsets (indexed by read id) and codes of the segment
+    const int32_t *cmin; int32_t cmin_len;
+    int32_t *hits;                                // out: PB200_HIT_INTS ints per hit {adapter, record}, at the append position
+    int32_t *next_active;                         // out: the read id at the append position
+    unsigned *count;                              // append counter (= hits of the round)
+    unsigned long long *max_len;                  // longest appended read (sizes the next round's DP launch)
+};
+constexpr int PB_HIT_INTS = 1 + PB_REC;
+constexpr uint8_t PB_CODE_N = 4u << 4;
+__global__ void middle_decide_kernel(const MiddleArgs a, int *__restrict__ status) {
+    const int lane = threadIdx.x & 31;
+    const int64_t warps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    int ovf = 0;
+    for (int64_t i = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < a.n; i += warps) {
+        const int64_t s = a.active ? (int64_t)a.active[i] : a.first + i;
+        const int32_t k0 = a.active ? a.next_ad[s] : 0;
+        const int32_t *rec = a.records + (size_t)s * a.n_adapters * PB_REC;
+        int hit = 0x7fffffff;
+        for (int32_t kb = k0; kb < a.n_adapters && hit == 0x7fffffff; kb += 32) {
+            const int32_t k = kb + lane;
+            int mine = 0x7fffffff;
+            if (k < a.n_adapters) {
+                int32_t r[PB_REC];
+#pragma unroll
+                for (int q = 0; q < PB_REC; ++q) r[q] = rec[(size_t)k * PB_REC + q];
+                if (middle_hit(r, a.cmin, a.cmin_len, &ovf)) mine = k;
+            }
+            hit = __reduce_min_sync(0xffffffffu, mine);
+        }
+        if (hit == 0x7fffffff) continue;              // warp-uniform: the read leaves the active set
+        const int32_t *r = rec + (size_t)hit * PB_REC;
+        const int64_t o0 = a.seq_off[s], len = a.seq_off[s + 1] - o0;
+        const int32_t rs = r[0], re = r[1];
+        if (rs < 0 || re < rs || re >= len) { ovf = 1; continue; }
+        for (int64_t p = rs + lane; p <= re; p += 32) a.codes[o0 + p] = PB_CODE_N;
+        unsigned pos = 0;
+        if (lane == 0) {
+            pos = atomicAdd(a.count, 1u);
+            atomicMax(a.max_len, (unsigned long long)len);
+            a.next_ad[s] = hit;
+            a.next_active[pos] = (int32_t)s;
+        }
+        pos = __shfl_sync(0xffffffffu, pos, 0);
+        if (lane < PB_HIT_INTS) a.hits[(size_t)pos * PB_HIT_INTS + lane] = lane == 0 ? hit : r[lane - 1];
     }
     if (ovf) atomicOr(status, 2);
 }

@@ -16,6 +16,8 @@ buffers end to end:
   trimmed_ranges(...)        the `seq[start_trim : len - end_trim]` slice of every read (Python slice semantics)
   find_middle_hits(...)      Phase C on the trimmed reads: one cross-product submit, then only the reads with a hit
                              are masked and re-submitted (the reference's sequential masking, nanopore_read.py:210-243)
+                             -- or, with PB200_DEVICE_MIDDLE=1, one adapterMiddleScan call that runs every round on
+                             the device
   middle_trim_ranges(...)    hits -> the ranges the reference adds to `middle_trim_positions`
   emit(...)                  get_fastq / get_fasta of every read (split parts, numbering, --discard_middle,
                              --min_split_read_size, RNA T->U) as one bytes object, assembled with vectorised scatters
@@ -341,15 +343,25 @@ def trimmed_ranges(lens, start_trim, end_trim):
     return np.where(untouched, 0, a), np.where(untouched, lens, b)
 
 
-def find_middle_hits(batch, start_trim, end_trim, adapters, middle_threshold, scoring_scheme_vals):
+# The whole middle scan on the device (include/porechop_b200.h adapterMiddleScan): masking rounds included, one engine call,
+# the masked reads and the records of reads without a hit stay on the device.  Off by default.
+DEVICE_MIDDLE = os.environ.get('PB200_DEVICE_MIDDLE', '0') == '1'
+
+
+def find_middle_hits(batch, start_trim, end_trim, adapters, middle_threshold, scoring_scheme_vals, device=None):
     """Phase C.  adapters: list of (name, sequence) in the reference's order (porechop.py:541-548).
     Returns {read index: [(adapter position, read_start, read_end, full_score), ...]} in the order the reference finds
     them; coordinates are in the trimmed read.  Round 0 is one cross product over all trimmed reads; only reads with
-    a hit are masked with '-' and re-submitted (as a pair list) from the adapter that hit."""
+    a hit are masked with '-' and re-submitted (as a pair list) from the adapter that hit.
+    device (default: the module switch DEVICE_MIDDLE): one adapterMiddleScan call runs every round on the device instead;
+    the same dict comes back.  Inputs the device scan does not take (threshold <= 0, adapters with other bases than
+    A/C/G/T/U, scoring schemes outside the int16 kernels: PB200_ERR_ARG) use the rounds above."""
     n, n_ad = len(batch), len(adapters)
     hits = {}
     if n == 0 or n_ad == 0:
         return hits
+    if device is None:
+        device = DEVICE_MIDDLE
     a, b = trimmed_ranges(batch.lengths(), start_trim, end_trim)
     # the trimmed reads of the chunk go into the engine's pinned staging buffer (reused chunk after chunk, uploaded by DMA at
     # PCIe speed) when there is one: a gather into fresh pageable memory + its upload would take far longer than the device
@@ -357,6 +369,18 @@ def find_middle_hits(batch, start_trim, end_trim, adapters, middle_threshold, sc
     tbuf, toff = _gather_ranges(batch.seq, batch.seq_off[:-1] + a, batch.seq_off[:-1] + b,
                                 alloc=(lambda nbytes: pinned(0, nbytes)) if pinned is not None else None)
     abuf, aoff = W.pack_sequences([x[1] for x in adapters], offset_dtype=np.int32)
+    if device:
+        try:
+            n_hits, h = W.adapter_middle_scan(tbuf, toff, abuf, aoff, scoring_scheme_vals, middle_threshold)
+        except W.EngineError as e:
+            if e.code != W.ERR_ARG:
+                raise
+        else:
+            full, _, rs, re_ = scores_from_records(np.ascontiguousarray(h[:, 1:]))
+            reads = np.repeat(np.arange(n), n_hits)
+            for k in range(len(h)):
+                hits.setdefault(int(reads[k]), []).append((int(h[k, 0]), int(rs[k]), int(re_[k]), float(full[k])))
+            return hits
     rec = W.adapter_alignment_batch(tbuf, toff, abuf, aoff, scoring_scheme_vals)
     full, _, rs, re_ = (x.reshape(n, n_ad) for x in scores_from_records(rec))
     hit = full >= middle_threshold                           # NaN never hits, as in the reference
