@@ -290,14 +290,14 @@ void timed_end(Engine &E, cudaStream_t s, TimedLaunch &tl, bool on) {
 }
 
 template <int G, int R, bool HS>
-int launch_trace_variant(Engine &E, Stage &S, cudaStream_t stream, const TaskSrc &ts, int max_n,
-                         const uint8_t *seq_codes, const uint8_t *ad_codes, const Scoring &sc, int32_t *out, int *status) {
+int launch_trace_variant(Engine &E, Stage &S, cudaStream_t stream, const TaskSrc &ts, int max_n, const uint8_t *seq_codes,
+                         bool seq_ascii, const uint8_t *ad_codes, const Scoring &sc, int32_t *out, int *status) {
     constexpr int SPW = 32 / G;
     constexpr int WPS = TraceWords<R>::value;
     const int max_steps = max_n + G - 1;
     const int wpb = PB_WARPS_PER_BLOCK;
     const size_t hb_words = HS ? (size_t)SPW * max_n : 0;
-    const size_t smem_bytes = (size_t)wpb * (hb_words + PB_SCRATCH_WORDS) * 4;
+    const size_t smem_bytes = ((size_t)wpb * (hb_words + PB_SCRATCH_WORDS) + (seq_ascii ? PB_CODE_TAB_WORDS : 0)) * 4;
     auto kern = trace_kernel<G, R, HS>;
     int bps = 0;
     if (int rc = E.blocks_per_sm(reinterpret_cast<const void *>(kern), wpb * 32, smem_bytes, &bps)) return rc;
@@ -321,7 +321,7 @@ int launch_trace_variant(Engine &E, Stage &S, cudaStream_t stream, const TaskSrc
     TimedLaunch tl; bool on;
     timed_begin(E, stream, tl, on, E.next_trace_kind);
     kern<<<(unsigned)blocks, wpb * 32, smem_bytes, stream>>>(ts, seq_codes, ad_codes, sc, out, S.gtrace.as<uint32_t>(), max_steps,
-                                                              max_n, status);
+                                                              max_n, seq_ascii ? 1 : 0, status);
     timed_end(E, stream, tl, on);
     g_launches++;
     CK(cudaGetLastError());
@@ -329,20 +329,21 @@ int launch_trace_variant(Engine &E, Stage &S, cudaStream_t stream, const TaskSrc
 }
 
 template <int G, int R>
-int launch_trace(Engine &E, Stage &S, cudaStream_t stream, const TaskSrc &ts, int max_n,
-                 const uint8_t *seq_codes, const uint8_t *ad_codes, const Scoring &sc, int32_t *out, int *status) {
+int launch_trace(Engine &E, Stage &S, cudaStream_t stream, const TaskSrc &ts, int max_n, const uint8_t *seq_codes,
+                 bool seq_ascii, const uint8_t *ad_codes, const Scoring &sc, int32_t *out, int *status) {
     constexpr int SPW = 32 / G;
     if (max_n < 1) max_n = 1;
     // packed read bases of a slot are staged in shared memory when they fit (<= 12 KB per warp), else in global scratch
     const bool hs = g_opt.hbuf_mode == 1 ? true : g_opt.hbuf_mode == 2 ? false : ((size_t)SPW * max_n * 4 <= 12288);
-    if (hs && (size_t)PB_WARPS_PER_BLOCK * ((size_t)SPW * max_n + 4 + PB_SCRATCH_WORDS) * 4 <= E.smem_optin)
-        return launch_trace_variant<G, R, true>(E, S, stream, ts, max_n, seq_codes, ad_codes, sc, out, status);
-    return launch_trace_variant<G, R, false>(E, S, stream, ts, max_n, seq_codes, ad_codes, sc, out, status);
+    if (hs && ((size_t)PB_WARPS_PER_BLOCK * ((size_t)SPW * max_n + 4 + PB_SCRATCH_WORDS) + PB_CODE_TAB_WORDS) * 4 <= E.smem_optin)
+        return launch_trace_variant<G, R, true>(E, S, stream, ts, max_n, seq_codes, seq_ascii, ad_codes, sc, out, status);
+    return launch_trace_variant<G, R, false>(E, S, stream, ts, max_n, seq_codes, seq_ascii, ad_codes, sc, out, status);
 }
 
-int launch_trace_class(Engine &E, Stage &S, cudaStream_t stream, int cls, const TaskSrc &ts, int max_n,
-                       const uint8_t *seq_codes, const uint8_t *ad_codes, const Scoring &sc, int32_t *out, int *status) {
-#define PB_CASE(K, GG, RR) case K: return launch_trace<GG, RR>(E, S, stream, ts, max_n, seq_codes, ad_codes, sc, out, status);
+// seq_ascii: `seq_codes` holds the caller's ASCII bytes, which the trace kernel encodes as it stages them (single pass only)
+int launch_trace_class(Engine &E, Stage &S, cudaStream_t stream, int cls, const TaskSrc &ts, int max_n, const uint8_t *seq_codes,
+                       bool seq_ascii, const uint8_t *ad_codes, const Scoring &sc, int32_t *out, int *status) {
+#define PB_CASE(K, GG, RR) case K: return launch_trace<GG, RR>(E, S, stream, ts, max_n, seq_codes, seq_ascii, ad_codes, sc, out, status);
     switch (cls) {
         PB_CASE(0, 4, 5) PB_CASE(1, 4, 6) PB_CASE(2, 4, 7) PB_CASE(3, 4, 8)
         PB_CASE(4, 8, 5) PB_CASE(5, 8, 6) PB_CASE(6, 8, 7) PB_CASE(7, 8, 8)
@@ -413,11 +414,13 @@ int launch_encode(cudaStream_t stream, const uint8_t *in, uint8_t *out, int64_t 
 }
 
 // Run every task of one class; `ts` describes the tasks in slot order (explicit records or the cross product).
+// seq_ascii: the sequences are the caller's ASCII bytes (see single_pass_ascii); only the single-pass trace takes them.
 int run_class_tasks(Engine &E, Stage &S, cudaStream_t stream, int cls, int m_max, const TaskSrc &ts, int64_t max_n,
                     const uint8_t *seq_codes, const uint8_t *ad_codes, const Scoring &sc, const SchemeInfo &si,
-                    int32_t *out, int *status, unsigned long long *counter) {
+                    int32_t *out, int *status, unsigned long long *counter, bool seq_ascii = false) {
     const int64_t n_tasks = ts.n_tasks;
     if (n_tasks <= 0) return 0;
+    if (seq_ascii && max_n > g_opt.direct_max) return fail(PB200_ERR_INTERNAL, "ASCII sequences reached the two-pass path");
     if (g_opt.profile != 0 && ts.tasks == nullptr && ts.cls_ad != nullptr && ts.n_cls_ad >= 3 && (ts.n_cls_ad & 1) &&
         si.bounded && max_n > g_opt.direct_max) {
         // the score pass's query profile needs same-read slots: the paired adapters (one read, two adapters per slot) and the
@@ -434,7 +437,7 @@ int run_class_tasks(Engine &E, Stage &S, cudaStream_t stream, int cls, int m_max
     }
     int64_t W = si.bounded ? (int64_t)m_max + ((int64_t)m_max * si.wnum) / si.wden : (int64_t)1 << 40;
     const bool two_pass = si.bounded && max_n > g_opt.direct_max && W + 1 < max_n;
-    if (!two_pass) return launch_trace_class(E, S, stream, cls, ts, (int)max_n, seq_codes, ad_codes, sc, out, status);
+    if (!two_pass) return launch_trace_class(E, S, stream, cls, ts, (int)max_n, seq_codes, seq_ascii, ad_codes, sc, out, status);
     if (int rc = S.ends.ensure((size_t)n_tasks * sizeof(EndCell))) return rc;
     if (int rc = S.tasks2.ensure((size_t)n_tasks * sizeof(Task))) return rc;
     if (int rc = launch_score_class(E, stream, cls, ts, counter, seq_codes, ad_codes, sc, S.ends.as<EndCell>())) return rc;
@@ -452,7 +455,7 @@ int run_class_tasks(Engine &E, Stage &S, cudaStream_t stream, int cls, int m_max
     TaskSrc t2 = ts;
     t2.tasks = S.tasks2.as<Task>();
     E.next_trace_kind = TK_TRACE_WINDOW;
-    const int rc2 = launch_trace_class(E, S, stream, cls, t2, (int)W, seq_codes, ad_codes, sc, out, status);
+    const int rc2 = launch_trace_class(E, S, stream, cls, t2, (int)W, seq_codes, false, ad_codes, sc, out, status);
     E.next_trace_kind = TK_TRACE;
     return rc2;
 }
@@ -590,10 +593,11 @@ int run_generic_cross(Engine &E, Stage &S, cudaStream_t stream, const ClassPlan 
 // d_seq_off points at the offset of sequence s0 (cnt+1 entries), base_off is subtracted from every offset.
 // seq_order (optional): slot i is sequence seq_order[i] of d_seq_off (the active reads of a middle-scan round); without it
 // the two-pass path orders the sequences longest first itself.
+// seq_ascii: `seq_codes` holds the caller's ASCII bytes; only when single_pass_ascii(P, max_n) holds.
 int run_cross_chunk(Engine &E, Stage &S, cudaStream_t stream, const AdapterPlan &P, const uint8_t *seq_codes,
                     const int64_t *d_seq_off, int64_t cnt, int64_t base_off, int64_t max_n, int32_t n_adapters,
                     int32_t *d_out, const int64_t *h_seq_off_abs, int64_t s0, const int32_t *h_ad_off,
-                    const int32_t *seq_order = nullptr) {
+                    const int32_t *seq_order = nullptr, bool seq_ascii = false) {
     if (int rc = S.misc.ensure(64)) return rc;
     int *status = S.misc.as<int>();
     unsigned long long *counter = reinterpret_cast<unsigned long long *>(S.misc.as<char>() + 16);
@@ -617,6 +621,7 @@ int run_cross_chunk(Engine &E, Stage &S, cudaStream_t stream, const AdapterPlan 
         cls_pos += C.ad_ids.size();
         if (C.cls == GENERIC_CLASS) {
             if (!h_seq_off_abs) return fail(PB200_ERR_INTERNAL, "generic class needs host offsets");
+            if (seq_ascii) return fail(PB200_ERR_INTERNAL, "ASCII sequences reached the generic class");
             if (int rc = run_generic_cross(E, S, stream, C, h_seq_off_abs, s0, cnt, base_off, h_ad_off, n_adapters, seq_codes,
                                            P.d_ad_codes, P.sc, d_out)) return rc;
             continue;
@@ -630,9 +635,18 @@ int run_cross_chunk(Engine &E, Stage &S, cudaStream_t stream, const AdapterPlan 
         if (ts.n_tasks == 0) continue;
         (void)base_off;
         if (int rc = run_class_tasks(E, S, stream, C.cls, C.m_max, ts, max_n, seq_codes, P.d_ad_codes, P.sc,
-                                     P.si, d_out, status, counter)) return rc;
+                                     P.si, d_out, status, counter, seq_ascii)) return rc;
     }
     return 0;
+}
+
+// True when every class of the plan runs through the single-pass trace kernel at reads of up to max_n bases (no generic
+// class, no score pass): the trace kernel then encodes the caller's ASCII bytes as it stages them, and the encode pass over
+// the batch (a read and a write of every byte) and its code buffer are not needed.
+bool single_pass_ascii(const AdapterPlan &P, int64_t max_n) {
+    if (max_n > g_opt.direct_max) return false;
+    for (const ClassPlan &C : P.classes) if (C.cls == GENERIC_CLASS) return false;
+    return true;
 }
 
 int check_status(Stage &S, cudaStream_t stream) {
@@ -932,9 +946,11 @@ int run_cross_jobs(Engine &E, std::vector<CrossJob> &jobs, int ma, int mi, int g
             NvtxRange r("pb200:stage_wait");
             CK(cudaStreamSynchronize(stream));   // previous use of this stage's buffers is complete
         }
+        // a chunk uploaded as ASCII that only the single-pass trace reads is staged from the raw bytes (no encode pass)
+        const bool ascii = !J.mid && it.buf < 0 && single_pass_ascii(P, c.max_n);
         if (int rc = S.seq_raw.ensure((size_t)bytes + 16)) return rc;
         if (!J.mid) {
-            if (int rc = S.seq_codes.ensure((size_t)bytes + 16)) return rc;
+            if (int rc = ascii ? 0 : S.seq_codes.ensure((size_t)bytes + 16)) return rc;
             if (int rc = S.out.ensure((size_t)cnt * J.n_adapters * PB_REC * 4)) return rc;
         }
         if (int rc = S.seq_off.ensure((size_t)(cnt + 1) * 8)) return rc;
@@ -953,7 +969,7 @@ int run_cross_jobs(Engine &E, std::vector<CrossJob> &jobs, int ma, int mi, int g
         }
         NvtxRange dp_range("pb200:dp");
         const int64_t mid_rel = J.mid ? base - J.seq_off[0] : 0;     // the chunk's first byte in the segment's resident codes
-        uint8_t *codes = J.mid ? J.mid->codes + mid_rel : S.seq_codes.as<uint8_t>();
+        uint8_t *codes = J.mid ? J.mid->codes + mid_rel : ascii ? S.seq_raw.as<uint8_t>() : S.seq_codes.as<uint8_t>();
         int32_t *recs = J.mid ? J.mid->rec + (size_t)s0 * J.n_adapters * PB_REC : S.out.as<int32_t>();
         if (c.uniform) stride_offsets_kernel<<<(unsigned)((cnt + 1 + 255) / 256), 256, 0, stream>>>(S.seq_off.as<int64_t>(), cnt + 1, c.max_n);
         else rebase_kernel<<<(unsigned)((cnt + 1 + 255) / 256), 256, 0, stream>>>(S.seq_off.as<int64_t>(), cnt + 1, base);
@@ -965,11 +981,11 @@ int run_cross_jobs(Engine &E, std::vector<CrossJob> &jobs, int ma, int mi, int g
         }
         if (it.buf >= 0) {
             if (int rc = launch_unpack(stream, S.seq_raw.as<uint8_t>(), codes, bytes, E.sm_count)) return rc;
-        } else {
+        } else if (!ascii) {
             if (int rc = launch_encode(stream, S.seq_raw.as<uint8_t>(), codes, bytes, E.sm_count)) return rc;
         }
         if (int rc = run_cross_chunk(E, S, stream, P, codes, S.seq_off.as<int64_t>(), cnt, base, c.max_n,
-                                     J.n_adapters, recs, J.seq_off, s0, J.ad_off)) return rc;
+                                     J.n_adapters, recs, J.seq_off, s0, J.ad_off, nullptr, ascii)) return rc;
         if (J.mid) {
             if (int rc = launch_middle_decide(E, stream, *J.mid, J.n_adapters, nullptr, s0, cnt, J.mid->active[0],
                                               S.misc.as<int>())) return rc;
@@ -1339,14 +1355,21 @@ int batch_device(const uint8_t *d_seqs, const int64_t *d_seq_off, int64_t n_seqs
     NvtxRange submit_range("pb200:submit_device");
     AdapterPlan P;
     if (int rc = plan_adapters(E, stream, adapters, ad_off, n_adapters, ma, mi, go, ge, P)) return rc;
-    if (int rc = S.seq_codes.ensure((size_t)total_seq_bytes + 16)) return rc;
-    if (int rc = launch_encode(stream, d_seqs, S.seq_codes.as<uint8_t>(), total_seq_bytes, E.sm_count)) return rc;
+    const bool fresh_misc = S.misc.p == nullptr;
     if (int rc = S.misc.ensure(64)) return rc;
-    CK(cudaMemsetAsync(S.misc.as<char>() + 16, 0, 48, stream));   // status word (offset 0) is sticky until pb200Synchronize
+    // status word (offset 0) is sticky until pb200Synchronize, which clears it; a newly allocated word starts at zero too
+    CK(cudaMemsetAsync(S.misc.as<char>() + (fresh_misc ? 0 : 16), 0, fresh_misc ? 64 : 48, stream));
     if (max_seq_len < 0) {
         if (int rc = device_max_len(S, stream, d_seq_off, n_seqs, &max_seq_len)) return rc;
     }
     if (max_seq_len > 0x7fff0000ll) return fail(PB200_ERR_ARG, "sequence longer than 2^31");
+    const bool ascii = single_pass_ascii(P, max_seq_len);
+    const uint8_t *seqs = d_seqs;
+    if (!ascii) {
+        if (int rc = S.seq_codes.ensure((size_t)total_seq_bytes + 16)) return rc;
+        if (int rc = launch_encode(stream, d_seqs, S.seq_codes.as<uint8_t>(), total_seq_bytes, E.sm_count)) return rc;
+        seqs = S.seq_codes.as<uint8_t>();
+    }
     std::vector<int64_t> h_off;   // only fetched when a generic class exists
     for (auto &c : P.classes) if (c.cls == GENERIC_CLASS) {
         h_off.resize((size_t)n_seqs + 1);
@@ -1357,9 +1380,9 @@ int batch_device(const uint8_t *d_seqs, const int64_t *d_seq_off, int64_t n_seqs
     int64_t max_cnt = std::max<int64_t>(1, g_opt.device_chunk_tasks / std::max<int32_t>(n_adapters, 1));
     for (int64_t s0 = 0; s0 < n_seqs; s0 += max_cnt) {
         const int64_t cnt = std::min(max_cnt, n_seqs - s0);
-        if (int rc = run_cross_chunk(E, S, stream, P, S.seq_codes.as<uint8_t>(), d_seq_off + s0, cnt, 0, max_seq_len,
+        if (int rc = run_cross_chunk(E, S, stream, P, seqs, d_seq_off + s0, cnt, 0, max_seq_len,
                                      n_adapters, d_out + (size_t)s0 * n_adapters * PB_REC,
-                                     h_off.empty() ? nullptr : h_off.data(), s0, ad_off)) return rc;
+                                     h_off.empty() ? nullptr : h_off.data(), s0, ad_off, nullptr, ascii)) return rc;
     }
     return 0;
 }

@@ -19,8 +19,17 @@
 namespace pb {
 
 constexpr int PB_WARPS_PER_BLOCK = 4;
+// trace_kernel blocks per SM.  Groups of G <= 8 lanes: 6 (80 registers), which the default trace scratch and the shared
+// memory hold for end windows (the scratch of a warp grows with G: 128 MB holds 6 blocks per SM of G = 4 / 8 at 150 columns,
+// 5 of G = 16 / 32).  The end-trim classes then spill, but only values of the slot set-up, the final-column scout and the
+// traceback; the hot 4-step chunk stays spill-free and no longer (DESIGN.md section 4).  On an H100 80GB HBM3 at a 700 W
+// power limit the end-trim launches ran 2.9 % faster than at 5 blocks.  Wider groups keep 5 blocks (96 registers): a sixth
+// block would not fit their scratch.
 #ifndef PB_TRACE_MIN_BLOCKS
-#define PB_TRACE_MIN_BLOCKS 5
+#define PB_TRACE_MIN_BLOCKS 6
+#endif
+#ifndef PB_TRACE_MIN_BLOCKS_WIDE
+#define PB_TRACE_MIN_BLOCKS_WIDE 5
 #endif
 constexpr int PB_SCRATCH_WORDS = 32 * 2 * 6;   // ScoutCand per lane per half
 constexpr int PB_TCHUNK = 4;                   // trace steps per 128-bit store (must stay 4: uint4)
@@ -231,16 +240,39 @@ __device__ __forceinline__ uint32_t pack_bases(uint32_t bA, uint32_t bB) {
 }
 
 // Stage the packed read bases of a slot's columns: hbuf[c] = pack_bases(A[c], B[c]) for c < nmax, PB_PAD_H past the end
-// of a half.  Each lane of the group builds every G-th column from single-byte streaming loads.
+// of a half.  Each lane of the group builds every G-th column from single-byte streaming loads, PB_STAGE_COLS columns at a
+// time with all their loads issued before any of them is used.  `ascii` (launch-uniform): the sequence buffer holds the
+// caller's bytes, and each one is encoded by a lookup in `code_tab` (shared memory, encode_byte of every byte value), so a
+// single-pass launch needs no encode pass over the whole batch.  (Calling encode_byte here instead, a chain of compares and
+// selects per byte, made the end-trim launches 0.27 ms per step slower: more than the encode pass they replace.)
 // (Walking the window in 16-column blocks with one aligned 128-bit load per half and block, funnel-shifted into place, was
 // slower: the shift / extract / bounds work per column outweighs the saved LSU instructions, so the byte loads stay.)
+constexpr int PB_STAGE_COLS = 4;
+constexpr int PB_CODE_TAB_WORDS = 256 / 4;
 template <int G>
 __device__ __forceinline__ void stage_columns(uint32_t *hbuf, int g, const uint8_t *seqA, int nA, const uint8_t *seqB, int nB,
-                                              int nmax) {
-    for (int c = g; c < nmax; c += G) {
-        const uint32_t bA = (c < nA) ? (uint32_t)__ldcs(seqA + c) : (uint32_t)PB_PAD_H;
-        const uint32_t bB = (c < nB) ? (uint32_t)__ldcs(seqB + c) : (uint32_t)PB_PAD_H;
-        hbuf[c] = pack_bases(bA, bB);
+                                              int nmax, bool ascii, const uint8_t *code_tab) {
+    for (int c0 = g; c0 < nmax; c0 += PB_STAGE_COLS * G) {
+        uint32_t bA[PB_STAGE_COLS], bB[PB_STAGE_COLS];
+#pragma unroll
+        for (int k = 0; k < PB_STAGE_COLS; ++k) {
+            const int c = c0 + k * G;
+            bA[k] = (c < nA) ? (uint32_t)__ldcs(seqA + c) : (uint32_t)PB_PAD_H;
+            bB[k] = (c < nB) ? (uint32_t)__ldcs(seqB + c) : (uint32_t)PB_PAD_H;
+        }
+        if (ascii) {
+#pragma unroll
+            for (int k = 0; k < PB_STAGE_COLS; ++k) {
+                const int c = c0 + k * G;
+                if (c < nA) bA[k] = code_tab[bA[k]];
+                if (c < nB) bB[k] = code_tab[bB[k]];
+            }
+        }
+#pragma unroll
+        for (int k = 0; k < PB_STAGE_COLS; ++k) {
+            const int c = c0 + k * G;
+            if (c < nmax) hbuf[c] = pack_bases(bA[k], bB[k]);
+        }
     }
 }
 
@@ -253,13 +285,23 @@ __device__ __forceinline__ void stage_columns(uint32_t *hbuf, int g, const uint8
 // (Measured and removed: a score-only first pass + bounded trace window for 150-column windows, and shared-memory query
 // profiles for the substitution operands -- neither beat this single pass.)
 template <int G, int R, bool HBUF_SMEM>
-__global__ void __launch_bounds__(PB_WARPS_PER_BLOCK * 32, PB_TRACE_MIN_BLOCKS)
+__global__ void __launch_bounds__(PB_WARPS_PER_BLOCK * 32, G <= 8 ? PB_TRACE_MIN_BLOCKS : PB_TRACE_MIN_BLOCKS_WIDE)
 trace_kernel(const TaskSrc ts, const uint8_t *__restrict__ seq,
              const uint8_t *__restrict__ ads, Scoring sc, int32_t *__restrict__ out, uint32_t *__restrict__ gtrace,
-             int max_steps, int max_n, int *__restrict__ status) {
+             int max_steps, int max_n, int seq_ascii, int *__restrict__ status) {
     constexpr int SPW = 32 / G;
     constexpr int WPS = TraceWords<R>::value;
     extern __shared__ uint32_t smem[];
+    // Shared memory: [ASCII input only: code table, byte value v -> encode_byte(v), PB_CODE_TAB_WORDS] then the per-warp
+    // regions (below).  The table is written once per block, before the slot loop.
+    const uint8_t *code_tab = reinterpret_cast<const uint8_t *>(smem);
+    if (seq_ascii) {
+        for (int w = threadIdx.x; w < PB_CODE_TAB_WORDS; w += blockDim.x)
+            smem[w] = encode_byte(4u * w) | (encode_byte(4u * w + 1) << 8) | (encode_byte(4u * w + 2) << 16) |
+                      (encode_byte(4u * w + 3) << 24);
+        __syncthreads();
+    }
+    uint32_t *const warp_smem = smem + (seq_ascii ? PB_CODE_TAB_WORDS : 0);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int grp = lane / G, g = lane % G;
     const int warps_per_block = blockDim.x >> 5;
@@ -281,7 +323,7 @@ trace_kernel(const TaskSrc ts, const uint8_t *__restrict__ seq,
     uint32_t *tr = gw;
     const int hb_words = HBUF_SMEM ? SPW * max_n : 0;
     const int per_warp_words = hb_words + PB_SCRATCH_WORDS;
-    uint32_t *wsm = smem + (size_t)warp * per_warp_words;
+    uint32_t *wsm = warp_smem + (size_t)warp * per_warp_words;
     uint32_t *hbuf = HBUF_SMEM ? (wsm + grp * max_n) : (gw + trace_words + (size_t)grp * max_n);
     ScoutCand *cand = reinterpret_cast<ScoutCand *>(wsm + hb_words);  // [half][lane]
     for (int64_t ws = wglobal; ws < n_wslots; ws += total_warps) {
@@ -295,7 +337,7 @@ trace_kernel(const TaskSrc ts, const uint8_t *__restrict__ seq,
             const Task tB = get_task(ts, slot * 2 + 1);
             nA = tA.n; nB = tB.n; mA = tA.m; mB = tB.m;
             nmax = max(nA, nB);
-            stage_columns<G>(hbuf, g, seq + tA.seq_off, nA, seq + tB.seq_off, nB, nmax);
+            stage_columns<G>(hbuf, g, seq + tA.seq_off, nA, seq + tB.seq_off, nB, nmax, seq_ascii != 0, code_tab);
             lane_init<R>(L, g, G, sc, ads + tA.ad_off, mA, (tA.flags & TASK_LEFT_INF) != 0, ads + tB.ad_off, mB,
                          (tB.flags & TASK_LEFT_INF) != 0);
             // scout: fast path while both halves are in inner columns; an empty half never limits it
