@@ -108,9 +108,15 @@ int pb200TrimThresholdTable(double end_threshold, int32_t len, int32_t *cmin);
 /* Same, with the bulk data already resident in device memory (d_seqs, d_seq_off, d_out are device pointers on
  * the current device; adapters/ad_off stay host pointers -- a few KB).  Cross-product mode only.
  * max_seq_len: length of the longest sequence, or -1 to let the library compute it on the device.
- * The work is enqueued on `stream` (a cudaStream_t passed as void*, NULL = the library's own stream) and the
- * call returns after enqueueing everything unless the score pass needs a host decision; call
- * cudaStreamSynchronize / torch.cuda.synchronize before reading d_out. */
+ * The work is enqueued on `stream` (a cudaStream_t passed as void*) and the call returns after enqueueing everything
+ * unless the score pass needs a host decision; call cudaStreamSynchronize / torch.cuda.synchronize before reading d_out.
+ * The reads must be in place when `stream` reaches the call: work the caller queued on `stream` before the call is
+ * ordered before it.  NULL = the library's own stream, which first waits for the work queued so far on the legacy default
+ * stream (where torch and plain CUDA calls go when no stream is chosen); it does not wait for other streams of the caller.
+ * Engine calls are ordered among themselves whatever their streams: every later call of this library, on any stream or
+ * thread, waits for this one's queued work before it touches the engine's buffers.  Deferred errors (a traceback that left
+ * its window) stay in a status word until pb200Synchronize reports and clears them; later calls that check the word
+ * (adapterMiddleScanDevice and the host-buffer calls) report them too. */
 int adapterAlignmentBatchDevice(const uint8_t *d_seqs, const int64_t *d_seq_off, int64_t n_seqs,
                                 int64_t total_seq_bytes, int64_t max_seq_len, const uint8_t *adapters,
                                 const int32_t *ad_off, int32_t n_adapters, int matchScore, int mismatchScore,
@@ -134,8 +140,9 @@ int adapterMiddleScan(const uint8_t *seqs, const int64_t *seq_off, int64_t n_seq
                       int gapExtensionScore, double middle_threshold, int32_t *n_hits, int32_t *hits, int64_t hits_cap,
                       int64_t *n_total);
 /* Same, with seqs / seq_off in device memory (conventions of adapterAlignmentBatchDevice; the caller's sequences are not
- * modified: the masking works on the library's encoded copy).  The work is enqueued on `stream`; the outputs are host
- * buffers, so the call returns only after they are written. */
+ * modified: the masking works on the library's encoded copy).  The work is enqueued on `stream` (NULL: as above) after the
+ * work earlier calls of this library left queued on any stream; the outputs are host buffers, so the call returns only
+ * after they are written. */
 int adapterMiddleScanDevice(const uint8_t *d_seqs, const int64_t *d_seq_off, int64_t n_seqs, int64_t total_seq_bytes,
                             int64_t max_seq_len, const uint8_t *adapters, const int32_t *ad_off, int32_t n_adapters,
                             int matchScore, int mismatchScore, int gapOpenScore, int gapExtensionScore,

@@ -192,6 +192,14 @@ struct Engine {
     // per read, hit slots, two active lists, threshold table, append counter + longest appended read
     DevBuf mid_codes, mid_off, mid_rec, mid_next_ad, mid_hits, mid_active[2], mid_cmin, mid_ctr;
     std::shared_ptr<void> packer;        // Packer (below): the thread that plans and packs chunks ahead of the submit loop
+    // Ordering between calls: every entry point uses the stage buffers above (st[0]'s trace scratch, tasks, codes, status word),
+    // whatever stream it runs on.  A call that returns with work still queued (adapterAlignmentBatchDevice) records `last` on
+    // its stream; every later call's streams wait for it before they touch a buffer (order_after_last).  `last_pending` is
+    // cleared once a call has synchronised with that work.  `legacy` orders the library's own stream after the caller's work
+    // on the legacy default stream (stream argument NULL, library_stream).
+    cudaEvent_t last = nullptr, legacy = nullptr;
+    cudaStream_t last_stream = nullptr;
+    bool last_pending = false;
     // launch constants, queried once per (kernel, dynamic shared-memory size); all users hold `mu`.  The opt-in shared-memory
     // limit is a property of the KERNEL, not of a launch: it is only ever raised (a launch with less is always valid).
     std::map<std::pair<const void *, size_t>, int> bps_cache;
@@ -223,10 +231,51 @@ struct Engine {
         sm_count = prop.multiProcessorCount;
         smem_optin = prop.sharedMemPerBlockOptin;
         for (int i = 0; i < NSTAGE; ++i) CK(cudaStreamCreateWithFlags(&st[i].stream, cudaStreamNonBlocking));
+        CK(cudaEventCreateWithFlags(&last, cudaEventDisableTiming));
+        CK(cudaEventCreateWithFlags(&legacy, cudaEventDisableTiming));
         init_done = true;
         return 0;
     }
 };
+
+// cudaStreamWaitEvent: `s` waits on the device for the work `e` captured.  Every CUDA runtime has it; a host stand-in of the
+// runtime that runs streams synchronously (an older tests/sim) may not, and then the overload below -- the stronger
+// host-side wait for the event -- is chosen instead.  Likewise a runtime header without the legacy-stream handle gets
+// stream 0, which is the legacy default stream in this library's builds (no per-thread default stream).
+template <class S, class Ev>
+auto stream_wait_event(S s, Ev e, int) -> decltype(cudaStreamWaitEvent(s, e, 0u)) { return cudaStreamWaitEvent(s, e, 0u); }
+template <class S, class Ev>
+cudaError_t stream_wait_event(S, Ev e, long) { return cudaEventSynchronize(e); }
+#ifndef cudaStreamLegacy
+#define cudaStreamLegacy ((cudaStream_t)0)
+#endif
+
+// `s` waits for the work an earlier call left queued on another stream (Engine::last).  Same stream: nothing to do, so a
+// caller that keeps to one stream (bench.py) runs exactly as before.
+int order_after_last(Engine &E, cudaStream_t s) {
+    if (E.last_pending && E.last_stream != s) CK(stream_wait_event(s, E.last, 0));
+    return 0;
+}
+int order_stages_after_last(Engine &E) {
+    for (int i = 0; i < NSTAGE; ++i) if (int rc = order_after_last(E, E.st[i].stream)) return rc;
+    return 0;
+}
+// the call's work on `s` is still queued when it returns: the next call waits for it
+int record_last(Engine &E, cudaStream_t s) {
+    CK(cudaEventRecord(E.last, s));
+    E.last_stream = s;
+    E.last_pending = true;
+    return 0;
+}
+// The stream of a device-resident call: the caller's, or for NULL the library's own stream (st[0]), which first waits for the
+// work queued so far on the legacy default stream -- where a caller that does not pick a stream has uploaded its reads.
+int library_stream(Engine &E, void *user_stream, cudaStream_t *s) {
+    if (user_stream) { *s = (cudaStream_t)user_stream; return 0; }
+    CK(cudaEventRecord(E.legacy, cudaStreamLegacy));
+    CK(stream_wait_event(E.st[0].stream, E.legacy, 0));
+    *s = E.st[0].stream;
+    return 0;
+}
 
 std::mutex g_engines_mu;
 std::map<int, std::unique_ptr<Engine>> g_engines;
@@ -412,6 +461,7 @@ int launch_encode(cudaStream_t stream, const uint8_t *in, uint8_t *out, int64_t 
     CK(cudaGetLastError());
     return 0;
 }
+
 
 // Run every task of one class; `ts` describes the tasks in slot order (explicit records or the cross product).
 // seq_ascii: the sequences are the caller's ASCII bytes (see single_pass_ascii); only the single-pass trace takes them.
@@ -655,6 +705,16 @@ int check_status(Stage &S, cudaStream_t stream) {
     CK(cudaStreamSynchronize(stream));
     if (st & 1) return fail(PB200_ERR_INTERNAL, "traceback left its window (window bound violated)");
     if (st & 2) return fail(PB200_ERR_INTERNAL, "decision kernel: value outside its table (len_aln >= table length or count > 65535)");
+    return 0;
+}
+
+// S.misc: status word at offset 0, score-pass counter at 16, max-length scratch at 32.  The status word is sticky until
+// pb200Synchronize, which reports and clears it: a deferred error of an earlier device-resident call must not be lost, so a
+// call clears the word only when it allocates it, and everything behind it always.
+int reset_misc(Stage &S, cudaStream_t stream) {
+    const bool fresh = S.misc.p == nullptr;
+    if (int rc = S.misc.ensure(64)) return rc;
+    CK(cudaMemsetAsync(S.misc.as<char>() + (fresh ? 0 : 16), 0, fresh ? 64 : 48, stream));
     return 0;
 }
 
@@ -902,10 +962,7 @@ struct Packer {
 // Caller holds E.mu and has run E.init().
 int run_cross_jobs(Engine &E, std::vector<CrossJob> &jobs, int ma, int mi, int go, int ge) {
     NvtxRange submit_range("pb200:submit");
-    for (int i = 0; i < NSTAGE; ++i) {
-        if (int rc = E.st[i].misc.ensure(64)) return rc;
-        CK(cudaMemsetAsync(E.st[i].misc.p, 0, 64, E.st[i].stream));
-    }
+    for (int i = 0; i < NSTAGE; ++i) if (int rc = reset_misc(E.st[i], E.st[i].stream)) return rc;
     int64_t total_bytes = 0;
     for (const CrossJob &J : jobs) if (J.n_seqs > 0 && J.n_adapters > 0) total_bytes += J.seq_off[J.n_seqs] - J.seq_off[0];
     const bool packed = pack_wanted(total_bytes);
@@ -1063,6 +1120,7 @@ int run_cross_jobs(Engine &E, std::vector<CrossJob> &jobs, int ma, int mi, int g
         cudaError_t e = cudaStreamSynchronize(E.st[i].stream);
         if (e != cudaSuccess && !rc_final) { rc_final = fail(PB200_ERR_CUDA, std::string("cudaStreamSynchronize: ") + cudaGetErrorString(e)); first_err = g_err; }
     }
+    E.last_pending = false;      // every stage waited for an earlier call's queued work and is now idle
     if (PK) {        // all uploads are complete: the pack buffers are free for the next submit
         std::lock_guard<std::mutex> lk(PK->mu);
         for (int i = 0; i < NPACK; ++i) PK->state[i] = Packer::FREE;
@@ -1089,14 +1147,14 @@ int batch_host(const uint8_t *seqs, const int64_t *seq_off, int64_t n_seqs, cons
     Engine &E = *Ep;
     std::lock_guard<std::mutex> lk(E.mu);
     if (int rc = E.init()) return rc;
-    if (cross) return run_cross_jobs(E, jobs, ma, mi, go, ge);
-
+    if (cross) {
+        if (int rc = order_stages_after_last(E)) return rc;
+        return run_cross_jobs(E, jobs, ma, mi, go, ge);
+    }
+    // pair-list mode runs on st[0] alone
+    if (int rc = order_after_last(E, E.st[0].stream)) return rc;
     AdapterPlan P;
     if (int rc = plan_adapters(E, E.st[0].stream, adapters, ad_off, n_adapters, ma, mi, go, ge, P)) return rc;
-    for (int i = 0; i < NSTAGE; ++i) {
-        if (int rc = E.st[i].misc.ensure(64)) return rc;
-        CK(cudaMemsetAsync(E.st[i].misc.p, 0, 64, E.st[i].stream));
-    }
 
     // ---- pair-list mode: all sequences resident, pairs ordered per class on the host ----
     auto run_pairs = [&]() -> int {
@@ -1111,8 +1169,7 @@ int batch_host(const uint8_t *seqs, const int64_t *seq_off, int64_t n_seqs, cons
     if (int rc = S.pair_seq.ensure((size_t)n_pairs * 4)) return rc;
     if (int rc = S.pair_ad.ensure((size_t)n_pairs * 4)) return rc;
     if (int rc = S.order.ensure((size_t)n_pairs * 4)) return rc;
-    if (int rc = S.misc.ensure(64)) return rc;
-    CK(cudaMemsetAsync(S.misc.p, 0, 64, stream));
+    if (int rc = reset_misc(S, stream)) return rc;
     if (bytes) CK(cudaMemcpyAsync(S.seq_raw.p, seqs, (size_t)bytes, cudaMemcpyHostToDevice, stream));
     CK(cudaMemcpyAsync(S.seq_off.p, seq_off, (size_t)(n_seqs + 1) * 8, cudaMemcpyHostToDevice, stream));
     CK(cudaMemcpyAsync(S.pair_seq.p, pair_seq, (size_t)n_pairs * 4, cudaMemcpyHostToDevice, stream));
@@ -1202,6 +1259,7 @@ int batch_host(const uint8_t *seqs, const int64_t *seq_off, int64_t n_seqs, cons
         cudaStreamSynchronize(E.st[0].stream);
         g_err = first_err;
     }
+    E.last_pending = false;                 // st[0] waited for an earlier call's queued work and is idle
     return rc_pairs;
 }
 
@@ -1224,6 +1282,7 @@ int batch_host_multi(const pb200_batch_t *batches, int n_batches, int ma, int mi
     Engine &E = *Ep;
     std::lock_guard<std::mutex> lk(E.mu);
     if (int rc = E.init()) return rc;
+    if (int rc = order_stages_after_last(E)) return rc;
     return run_cross_jobs(E, jobs, ma, mi, go, ge);
 }
 
@@ -1309,6 +1368,7 @@ int batch_end_decisions(const pb200_end_batch_t *batches, int n_batches, int ma,
     Engine &E = *Ep;
     std::lock_guard<std::mutex> lk(E.mu);
     if (int rc = E.init()) return rc;
+    if (int rc = order_stages_after_last(E)) return rc;
     cudaStream_t s0 = E.st[0].stream;
     for (size_t j = 0; j < jobs.size(); ++j) {
         const pb200_end_batch_t &D = *jobs[j].dec;
@@ -1339,6 +1399,10 @@ int device_max_len(Stage &S, cudaStream_t stream, const int64_t *d_seq_off, int6
     return 0;
 }
 
+int batch_device_queue(Engine &E, cudaStream_t stream, const uint8_t *d_seqs, const int64_t *d_seq_off, int64_t n_seqs,
+                       int64_t total_seq_bytes, int64_t max_seq_len, const uint8_t *adapters, const int32_t *ad_off,
+                       int32_t n_adapters, int ma, int mi, int go, int ge, int32_t *d_out);
+
 int batch_device(const uint8_t *d_seqs, const int64_t *d_seq_off, int64_t n_seqs, int64_t total_seq_bytes,
                  int64_t max_seq_len, const uint8_t *adapters, const int32_t *ad_off, int32_t n_adapters, int ma, int mi,
                  int go, int ge, int32_t *d_out, void *user_stream) {
@@ -1350,15 +1414,27 @@ int batch_device(const uint8_t *d_seqs, const int64_t *d_seq_off, int64_t n_seqs
     Engine &E = *Ep;
     std::lock_guard<std::mutex> lk(E.mu);
     if (int rc = E.init()) return rc;
+    cudaStream_t stream = nullptr;
+    if (int rc = library_stream(E, user_stream, &stream)) return rc;
+    if (int rc = order_after_last(E, stream)) return rc;
+    // the work is queued on `stream` and the call returns without waiting for it: whatever happens below, the next call
+    // must wait for what was queued
+    const int rc = batch_device_queue(E, stream, d_seqs, d_seq_off, n_seqs, total_seq_bytes, max_seq_len, adapters, ad_off,
+                                      n_adapters, ma, mi, go, ge, d_out);
+    const std::string first_err = g_err;
+    const int rc_last = record_last(E, stream);
+    if (rc) { g_err = first_err; return rc; }
+    return rc_last;
+}
+
+int batch_device_queue(Engine &E, cudaStream_t stream, const uint8_t *d_seqs, const int64_t *d_seq_off, int64_t n_seqs,
+                       int64_t total_seq_bytes, int64_t max_seq_len, const uint8_t *adapters, const int32_t *ad_off,
+                       int32_t n_adapters, int ma, int mi, int go, int ge, int32_t *d_out) {
     Stage &S = E.st[0];
-    cudaStream_t stream = user_stream ? (cudaStream_t)user_stream : S.stream;
     NvtxRange submit_range("pb200:submit_device");
     AdapterPlan P;
     if (int rc = plan_adapters(E, stream, adapters, ad_off, n_adapters, ma, mi, go, ge, P)) return rc;
-    const bool fresh_misc = S.misc.p == nullptr;
-    if (int rc = S.misc.ensure(64)) return rc;
-    // status word (offset 0) is sticky until pb200Synchronize, which clears it; a newly allocated word starts at zero too
-    CK(cudaMemsetAsync(S.misc.as<char>() + (fresh_misc ? 0 : 16), 0, fresh_misc ? 64 : 48, stream));
+    if (int rc = reset_misc(S, stream)) return rc;
     if (max_seq_len < 0) {
         if (int rc = device_max_len(S, stream, d_seq_off, n_seqs, &max_seq_len)) return rc;
     }
@@ -1384,6 +1460,12 @@ int batch_device(const uint8_t *d_seqs, const int64_t *d_seq_off, int64_t n_seqs
                                      n_adapters, d_out + (size_t)s0 * n_adapters * PB_REC,
                                      h_off.empty() ? nullptr : h_off.data(), s0, ad_off, nullptr, ascii)) return rc;
     }
+#ifdef PB_TEST_DEFERRED_STATUS
+    // tests of the host-simulated engine only (through PB200_SIM_FLAGS): the call's last operation sets the status word's
+    // "window bound violated" bit, as a trace kernel does when a traceback leaves its window, so that the deferred-error
+    // path of the device-resident API can be tested
+    CK(cudaMemsetAsync(S.misc.p, 1, 1, stream));
+#endif
     return 0;
 }
 
@@ -1554,6 +1636,7 @@ int middle_host(const uint8_t *seqs, const int64_t *seq_off, int64_t n_seqs, con
     Engine &E = *Ep;
     std::lock_guard<std::mutex> lk(E.mu);
     if (int rc = E.init()) return rc;
+    if (int rc = order_stages_after_last(E)) return rc;
     NvtxRange submit_range("pb200:submit_middle");
     Stage &S = E.st[0];
     cudaStream_t stream = S.stream;
@@ -1581,12 +1664,14 @@ int middle_host(const uint8_t *seqs, const int64_t *seq_off, int64_t n_seqs, con
         }
         return 0;
     };
-    if (int rc = run()) {                 // nothing may still be running when we return
+    const int rc = run();
+    if (rc) {                             // nothing may still be running when we return
         const std::string first_err = g_err;
         cudaStreamSynchronize(stream);
         g_err = first_err;
-        return rc;
     }
+    E.last_pending = false;               // the streams waited for an earlier call's queued work and are idle
+    if (rc) return rc;
     return middle_emit(rounds, n_seqs, n_hits, hits, hits_cap, n_total);
 }
 
@@ -1615,9 +1700,11 @@ int middle_device(const uint8_t *d_seqs, const int64_t *d_seq_off, int64_t n_seq
     Engine &E = *Ep;
     std::lock_guard<std::mutex> lk(E.mu);
     if (int rc = E.init()) return rc;
-    NvtxRange submit_range("pb200:submit_middle");
     Stage &S = E.st[0];
-    cudaStream_t stream = user_stream ? (cudaStream_t)user_stream : S.stream;
+    cudaStream_t stream = nullptr;
+    if (int rc = library_stream(E, user_stream, &stream)) return rc;
+    if (int rc = order_after_last(E, stream)) return rc;
+    NvtxRange submit_range("pb200:submit_middle");
     std::vector<MiddleRound> rounds;
     auto run = [&]() -> int {
         if (!S.misc.p) {
@@ -1657,12 +1744,14 @@ int middle_device(const uint8_t *d_seqs, const int64_t *d_seq_off, int64_t n_seq
         }
         return 0;
     };
-    if (int rc = run()) {
+    const int rc = run();
+    if (rc) {
         const std::string first_err = g_err;
         cudaStreamSynchronize(stream);
         g_err = first_err;
-        return rc;
     }
+    E.last_pending = false;
+    if (rc) return rc;
     return middle_emit(rounds, n_seqs, n_hits, hits, hits_cap, n_total);
 }
 
@@ -1830,6 +1919,7 @@ int pb200Synchronize(void) {
     std::lock_guard<std::mutex> lk(E.mu);
     if (!E.init_done) return 0;
     CK(cudaDeviceSynchronize());
+    E.last_pending = false;
     int rc_final = 0;
     for (int i = 0; i < NSTAGE; ++i) {
         if (!E.st[i].misc.p) continue;

@@ -1,6 +1,10 @@
 // tests/sim/pbsim.cpp -- block scheduler of the host CUDA stand-in (see pbsim_cuda.h).  TESTS ONLY.
 #include "pbsim_cuda.h"
 
+#include <memory>
+#include <mutex>
+#include <set>
+
 #if defined(__x86_64__) && !defined(PBSIM_NO_FAST_SWITCH)
 // swapcontext() saves and restores the signal mask with a system call on every switch; a fiber switch here only needs the
 // callee-saved registers and the stack pointer.
@@ -217,3 +221,166 @@ void run_grid(dim3 grid, dim3 block, size_t smem, const std::function<void()> &b
 }
 
 }  // namespace pbsim
+
+// ---- stream ordering: vector clocks, accesses, races (see pbsim_cuda.h) ---------------------------------------------
+namespace pbsim {
+namespace {
+
+typedef std::vector<unsigned> VC;
+void join(VC &a, const VC &b) {
+    if (a.size() < b.size()) a.resize(b.size(), 0);
+    for (size_t i = 0; i < b.size(); ++i) a[i] = std::max(a[i], b[i]);
+}
+unsigned at(const VC &v, int i) { return (size_t)i < v.size() ? v[(size_t)i] : 0; }
+
+struct StreamObj { int id; bool blocking; };
+struct EventObj { VC clock; };
+struct Access {
+    size_t lo, hi;                  // byte range inside the allocation
+    Acc kind;
+    int stream; unsigned epoch;     // the operation: its stream and that stream's clock component
+    std::shared_ptr<const std::string> op;
+    std::string what;
+};
+struct Alloc { size_t size; std::vector<Access> acc; };
+
+std::mutex mu;
+std::vector<VC> streams(1);         // [0] = the legacy default stream
+std::vector<bool> blocking(1, true);
+VC host;
+std::map<uintptr_t, Alloc> allocs;
+std::set<std::string> races;
+long long n_races = 0;
+thread_local int cur_stream = -1;
+thread_local VC cur_clock;
+thread_local std::shared_ptr<const std::string> cur_op;
+
+const char *kind_name(Acc k) { return k == ACC_READ ? "read" : k == ACC_WRITE ? "write" : "atomic"; }
+
+int stream_id(void *s) {            // NULL, cudaStreamLegacy and cudaStreamPerThread are the legacy stream here
+    if (s == nullptr || s == (void *)0x1 || s == (void *)0x2) return 0;
+    return static_cast<StreamObj *>(s)->id;
+}
+
+}  // namespace
+
+void *hb_stream_create(bool is_blocking) {
+    std::lock_guard<std::mutex> lk(mu);
+    StreamObj *o = new StreamObj{(int)streams.size(), is_blocking};
+    streams.emplace_back();
+    blocking.push_back(is_blocking);
+    return o;
+}
+void hb_stream_destroy(void *s) { (void)s; }   // ids stay valid: accesses of the stream may still be checked against
+
+void hb_op_begin(void *s, const std::string &what) {
+    std::lock_guard<std::mutex> lk(mu);
+    const int id = stream_id(s);
+    VC &c = streams[(size_t)id];
+    join(c, host);
+    if (id == 0) { for (size_t k = 1; k < streams.size(); ++k) if (blocking[k]) join(c, streams[k]); }
+    else if (blocking[(size_t)id]) join(c, streams[0]);
+    if (c.size() <= (size_t)id) c.resize((size_t)id + 1, 0);
+    c[(size_t)id]++;
+    cur_stream = id;
+    cur_clock = c;
+    cur_op = std::make_shared<const std::string>(what + " [stream " + std::to_string(id) + "]");
+}
+void hb_op_end() { cur_stream = -1; cur_op.reset(); }
+
+void hb_access(const void *p, size_t bytes, Acc kind, const std::string &what) {
+    if (cur_stream < 0 || p == nullptr) return;
+    std::lock_guard<std::mutex> lk(mu);
+    const uintptr_t a = reinterpret_cast<uintptr_t>(p);
+    auto it = allocs.upper_bound(a);
+    if (it == allocs.begin()) return;
+    --it;
+    Alloc &A = it->second;
+    if (a >= it->first + A.size) return;            // not device memory of this library (host memory, caller's buffers)
+    const size_t lo = a - it->first;
+    const size_t hi = bytes == 0 ? lo + 1 : bytes == (size_t)-1 || bytes > A.size - lo ? A.size : lo + bytes;
+    // accesses the host has synchronised with happen before every later operation: drop them
+    A.acc.erase(std::remove_if(A.acc.begin(), A.acc.end(), [](const Access &x) { return at(host, x.stream) >= x.epoch; }),
+                A.acc.end());
+    for (const Access &x : A.acc) {
+        if (x.stream == cur_stream || at(cur_clock, x.stream) >= x.epoch) continue;      // ordered
+        if (x.hi <= lo || hi <= x.lo) continue;
+        if (x.kind == ACC_READ && kind == ACC_READ) continue;
+        if (x.kind == ACC_ATOMIC && kind == ACC_ATOMIC) continue;
+        ++n_races;
+        races.insert("race on a " + std::to_string(A.size) + "-byte allocation, bytes [" + std::to_string(std::max(lo, x.lo)) +
+                     ", " + std::to_string(std::min(hi, x.hi)) + "):\n  " + kind_name(x.kind) + " of " + x.what + " by " + *x.op +
+                     "\n  " + kind_name(kind) + " of " + what + " by " + *cur_op);
+    }
+    A.acc.push_back(Access{lo, hi, kind, cur_stream, at(cur_clock, cur_stream), cur_op, what});
+}
+
+void hb_malloc(void *p, size_t n) {
+    std::lock_guard<std::mutex> lk(mu);
+    allocs[reinterpret_cast<uintptr_t>(p)] = Alloc{n, {}};
+}
+void hb_sync_device() {
+    std::lock_guard<std::mutex> lk(mu);
+    for (const VC &c : streams) join(host, c);
+}
+void hb_free(void *p) {
+    hb_sync_device();                                // cudaFree synchronises the device
+    std::lock_guard<std::mutex> lk(mu);
+    allocs.erase(reinterpret_cast<uintptr_t>(p));
+}
+void hb_sync_stream(void *s) {
+    std::lock_guard<std::mutex> lk(mu);
+    const int id = stream_id(s);
+    join(host, streams[(size_t)id]);
+    if (id == 0) for (size_t k = 1; k < streams.size(); ++k) if (blocking[k]) join(host, streams[k]);
+}
+void *hb_event_create() { return new EventObj(); }
+void hb_event_destroy(void *e) { delete static_cast<EventObj *>(e); }
+void hb_event_record(void *e, void *s) {
+    if (!e) return;
+    hb_op_begin(s, "cudaEventRecord");
+    hb_op_end();
+    std::lock_guard<std::mutex> lk(mu);
+    static_cast<EventObj *>(e)->clock = streams[(size_t)stream_id(s)];
+}
+void hb_event_sync(void *e) {
+    if (!e) return;
+    std::lock_guard<std::mutex> lk(mu);
+    join(host, static_cast<EventObj *>(e)->clock);
+}
+void hb_stream_wait(void *s, void *e) {
+    if (!e) return;
+    std::lock_guard<std::mutex> lk(mu);
+    join(streams[(size_t)stream_id(s)], static_cast<EventObj *>(e)->clock);
+}
+
+std::string site_arg(const Site &s, int idx) {
+    const char *p = s.args;
+    for (int k = 0; k < idx && p; ++k) { p = strchr(p, '\037'); if (p) ++p; }
+    if (!p) return std::string(s.kernel) + " arg " + std::to_string(idx);
+    const char *e = strchr(p, '\037');
+    return std::string(s.kernel) + " arg `" + std::string(p, e ? (size_t)(e - p) : strlen(p)) + "`";
+}
+
+}  // namespace pbsim
+
+extern "C" {
+// a blocking stream (cudaStreamCreate) for tests that call the engine on streams of their own
+void *pbsim_stream_create(void) { return pbsim::hb_stream_create(true); }
+// "device" memory the check tracks, and an upload into it on a stream: a test's reads and records then take part in it
+void *pbsim_device_alloc(long long n) { void *p = nullptr; return cudaMalloc(&p, (size_t)n) == cudaSuccess ? p : nullptr; }
+void pbsim_device_free(void *p) { cudaFree(p); }
+void pbsim_upload(void *dst, const void *src, long long n, void *stream) {
+    cudaMemcpyAsync(dst, src, (size_t)n, cudaMemcpyHostToDevice, (cudaStream_t)stream);
+}
+long long pbsim_race_count(void) { std::lock_guard<std::mutex> lk(pbsim::mu); return pbsim::n_races; }
+void pbsim_race_clear(void) { std::lock_guard<std::mutex> lk(pbsim::mu); pbsim::n_races = 0; pbsim::races.clear(); }
+// the distinct races found since the last clear, one paragraph each; returns the length of the whole text (buf may be NULL)
+long long pbsim_race_report(char *buf, long long cap) {
+    std::lock_guard<std::mutex> lk(pbsim::mu);
+    std::string t;
+    for (const std::string &r : pbsim::races) t += r + "\n";
+    if (buf && cap > 0) { const size_t n = std::min((size_t)cap - 1, t.size()); memcpy(buf, t.data(), n); buf[n] = 0; }
+    return (long long)t.size();
+}
+}

@@ -18,6 +18,8 @@
 #include <algorithm>
 #include <functional>
 #include <map>
+#include <string>
+#include <type_traits>
 #include <vector>
 
 // ---- vector types / qualifiers ---------------------------------------------------------------------------
@@ -60,23 +62,76 @@ inline cudaError_t cudaGetDeviceProperties(cudaDeviceProp *p, int) {
     p->sharedMemPerBlockOptin = 227 * 1024;
     return cudaSuccess;
 }
-inline cudaError_t cudaMalloc(void **p, size_t n) { *p = malloc(n ? n : 1); return *p ? cudaSuccess : 2; }
+// ---- stream ordering: happens-before checking (pbsim.cpp) -----------------------------------------------------
+// Streams still execute synchronously, but every stream operation also gets the vector clock that CUDA guarantees for it:
+// join(its stream's clock, the host's clock) -- plus, on the legacy stream and on blocking streams, the implicit
+// synchronisation between the two -- and then a tick of its stream's own component.  cudaEventRecord captures a stream's
+// clock and cudaStreamWaitEvent joins it into another stream; the synchronise calls (and cudaFree, which synchronises the
+// device) join stream clocks into the host's.  Each operation's accesses to cudaMalloc'd memory are recorded, and two
+// accesses of different streams to overlapping bytes race when neither operation happens before the other and at least one
+// writes.  Atomics (64-bit counters, append slots) race only with plain accesses.  pbsim_race_count / _report / _clear
+// (extern "C") expose the races found.
+namespace pbsim {
+enum Acc { ACC_READ = 0, ACC_WRITE = 1, ACC_ATOMIC = 2 };
+void hb_op_begin(void *stream, const std::string &what);   // one operation of `stream`: its accesses follow, then hb_op_end
+void hb_access(const void *p, size_t bytes, Acc kind, const std::string &what);   // bytes = 0: the address p itself
+void hb_op_end();
+void hb_malloc(void *p, size_t n);
+void hb_free(void *p);
+void hb_sync_stream(void *stream);
+void hb_sync_device();
+void *hb_stream_create(bool blocking);
+void hb_stream_destroy(void *stream);
+void *hb_event_create();
+void hb_event_destroy(void *event);
+void hb_event_record(void *event, void *stream);
+void hb_event_sync(void *event);
+void hb_stream_wait(void *stream, void *event);
+}  // namespace pbsim
+#define cudaStreamLegacy ((cudaStream_t)0x1)
+#define cudaStreamPerThread ((cudaStream_t)0x2)
+inline cudaError_t cudaMalloc(void **p, size_t n) {
+    *p = malloc(n ? n : 1);
+    if (*p) pbsim::hb_malloc(*p, n ? n : 1);
+    return *p ? cudaSuccess : 2;
+}
 template <class T> inline cudaError_t cudaMalloc(T **p, size_t n) { return cudaMalloc(reinterpret_cast<void **>(p), n); }
-inline cudaError_t cudaFree(void *p) { free(p); return cudaSuccess; }
+inline cudaError_t cudaFree(void *p) { pbsim::hb_free(p); free(p); return cudaSuccess; }     // synchronises the device
 inline cudaError_t cudaHostAlloc(void **p, size_t n, unsigned) { *p = malloc(n ? n : 1); return *p ? cudaSuccess : 2; }
 inline cudaError_t cudaFreeHost(void *p) { free(p); return cudaSuccess; }
-inline cudaError_t cudaMemcpyAsync(void *d, const void *s, size_t n, cudaMemcpyKind, cudaStream_t = nullptr) { memcpy(d, s, n); return cudaSuccess; }
-inline cudaError_t cudaMemsetAsync(void *d, int v, size_t n, cudaStream_t = nullptr) { memset(d, v, n); return cudaSuccess; }
-inline cudaError_t cudaStreamCreateWithFlags(cudaStream_t *s, unsigned) { static char dummy[64]; static int k = 0; *s = dummy + (++k % 60) + 1; return cudaSuccess; }
-inline cudaError_t cudaStreamSynchronize(cudaStream_t) { return cudaSuccess; }
-inline cudaError_t cudaDeviceSynchronize() { return cudaSuccess; }
-inline cudaError_t cudaEventCreate(cudaEvent_t *e) { *e = nullptr; return cudaSuccess; }
+// the copy / memset calls are macros so that a race report can quote the call's arguments and line
+inline cudaError_t pbsim_memcpy_async(const char *args, const char *fn, int line, void *d, const void *s, size_t n, cudaMemcpyKind,
+                                      cudaStream_t st = nullptr) {
+    const std::string what = std::string("cudaMemcpyAsync(") + args + ") in " + fn + "(), line " + std::to_string(line);
+    pbsim::hb_op_begin(st, what);
+    pbsim::hb_access(s, n, pbsim::ACC_READ, "source");
+    pbsim::hb_access(d, n, pbsim::ACC_WRITE, "destination");
+    pbsim::hb_op_end();
+    memcpy(d, s, n);
+    return cudaSuccess;
+}
+inline cudaError_t pbsim_memset_async(const char *args, const char *fn, int line, void *d, int v, size_t n, cudaStream_t st = nullptr) {
+    pbsim::hb_op_begin(st, std::string("cudaMemsetAsync(") + args + ") in " + fn + "(), line " + std::to_string(line));
+    pbsim::hb_access(d, n, pbsim::ACC_WRITE, "destination");
+    pbsim::hb_op_end();
+    memset(d, v, n);
+    return cudaSuccess;
+}
+#define cudaMemcpyAsync(...) pbsim_memcpy_async(#__VA_ARGS__, __func__, __LINE__, __VA_ARGS__)
+#define cudaMemsetAsync(...) pbsim_memset_async(#__VA_ARGS__, __func__, __LINE__, __VA_ARGS__)
+inline cudaError_t cudaStreamCreateWithFlags(cudaStream_t *s, unsigned flags) { *s = pbsim::hb_stream_create(!(flags & 1u)); return cudaSuccess; }
+inline cudaError_t cudaStreamCreate(cudaStream_t *s) { *s = pbsim::hb_stream_create(true); return cudaSuccess; }
+inline cudaError_t cudaStreamDestroy(cudaStream_t s) { pbsim::hb_stream_destroy(s); return cudaSuccess; }
+inline cudaError_t cudaStreamSynchronize(cudaStream_t s) { pbsim::hb_sync_stream(s); return cudaSuccess; }
+inline cudaError_t cudaDeviceSynchronize() { pbsim::hb_sync_device(); return cudaSuccess; }
+inline cudaError_t cudaEventCreate(cudaEvent_t *e) { *e = pbsim::hb_event_create(); return cudaSuccess; }
 #define cudaEventDisableTiming 2u
-inline cudaError_t cudaEventCreateWithFlags(cudaEvent_t *e, unsigned) { *e = nullptr; return cudaSuccess; }
-inline cudaError_t cudaEventRecord(cudaEvent_t, cudaStream_t = nullptr) { return cudaSuccess; }
-inline cudaError_t cudaEventSynchronize(cudaEvent_t) { return cudaSuccess; }
+inline cudaError_t cudaEventCreateWithFlags(cudaEvent_t *e, unsigned) { *e = pbsim::hb_event_create(); return cudaSuccess; }
+inline cudaError_t cudaEventRecord(cudaEvent_t e, cudaStream_t s = nullptr) { pbsim::hb_event_record(e, s); return cudaSuccess; }
+inline cudaError_t cudaEventSynchronize(cudaEvent_t e) { pbsim::hb_event_sync(e); return cudaSuccess; }
+inline cudaError_t cudaStreamWaitEvent(cudaStream_t s, cudaEvent_t e, unsigned = 0) { pbsim::hb_stream_wait(s, e); return cudaSuccess; }
 inline cudaError_t cudaEventElapsedTime(float *ms, cudaEvent_t, cudaEvent_t) { *ms = 0.f; return cudaSuccess; }
-inline cudaError_t cudaEventDestroy(cudaEvent_t) { return cudaSuccess; }
+inline cudaError_t cudaEventDestroy(cudaEvent_t e) { pbsim::hb_event_destroy(e); return cudaSuccess; }
 // cudaFuncAttributeMaxDynamicSharedMemorySize is a property of the KERNEL (last value set wins); a launch asking for more
 // dynamic shared memory than the attribute (48 KB if never set) fails with "invalid argument" on the device -- reproduced here
 // (round 2: a per-size cache of the attribute call let a later, smaller value stand while a larger launch followed).
@@ -130,13 +185,38 @@ void poison_shared(void *p, size_t bytes);
 unsigned long long collective(Op op, unsigned mask, unsigned long long val, int arg, int width);
 void run_grid(dim3 grid, dim3 block, size_t smem, const std::function<void()> &body);
 
+// A launch site, filled in by build_sim.py: kernel name, its argument expressions (separated by \037), function and line.
+struct Site { const char *kernel, *args, *func; int line; };
+std::string site_arg(const Site &s, int idx);        // "kernel arg `expr`"
+
+// Kernel arguments as accesses: a `const T *` argument is a read and a `T *` argument a write of the data at the address it
+// points to (a kernel's extent is not known here: two launches handed the same buffer conflict, launches handed disjoint
+// pieces of one buffer do not); `unsigned long long *` arguments are the 64-bit atomic counters.  Pointers inside by-value
+// struct arguments are classified by pbsim_fields() -- overloads for the kernels' argument structs are in pbsim_fields.h.
+template <class T> inline void pbsim_fields(const T &, const std::string &) {}
+template <class T> inline void classify_arg(const T &v, const Site &s, int idx) {
+    if constexpr (std::is_pointer<T>::value) {
+        using P = typename std::remove_pointer<T>::type;
+        if (!v) return;
+        const Acc k = std::is_const<P>::value ? ACC_READ
+                    : std::is_same<typename std::remove_cv<P>::type, unsigned long long>::value ? ACC_ATOMIC : ACC_WRITE;
+        hb_access(reinterpret_cast<const void *>(v), 0, k, site_arg(s, idx));
+    } else {
+        pbsim_fields(v, site_arg(s, idx));
+    }
+}
+
 template <class F, class... Args>
-inline void launch(F f, dim3 grid, dim3 block, size_t smem, cudaStream_t, Args... args) {
+inline void launch(const Site &site, F f, dim3 grid, dim3 block, size_t smem, cudaStream_t stream, Args... args) {
     {   // the kernel's dynamic shared-memory limit: 48 KB unless the attribute was set -- then exactly that value
         auto it = pbsim_smem_attr().find(reinterpret_cast<const void *>(f));
         const size_t limit = it == pbsim_smem_attr().end() ? (size_t)48 * 1024 : it->second;
         if (smem > limit) { pbsim_last_error() = cudaErrorInvalidValue; return; }
     }
+    hb_op_begin(stream, std::string(site.kernel) + "<<<>>> in " + site.func + "(), line " + std::to_string(site.line));
+    int idx = 0;
+    (classify_arg(args, site, idx++), ...);
+    hb_op_end();
     run_grid(grid, block, smem, [=]() { f(args...); });
 }
 

@@ -15,6 +15,15 @@ from helpers import ROOT, oracle_batch
 sys.path.insert(0, os.path.join(ROOT, 'tests', 'sim'))
 
 
+@pytest.fixture(autouse=True)
+def _stream_order_checked():
+    """every test here also passes the simulated runtime's stream-ordering check (pbsim_cuda.h): no race between streams"""
+    import sim_engine
+    sim_engine.clear_races()
+    yield
+    sim_engine.assert_no_races()
+
+
 @pytest.fixture(scope='module')
 def W():
     import sim_engine

@@ -18,6 +18,15 @@ from test_oracle import SURVEY_EDGE, rebuild_fullread_inputs
 
 sys.path.insert(0, os.path.join(ROOT, 'tests', 'sim'))
 
+@pytest.fixture(autouse=True)
+def _stream_order_checked():
+    """every test here also passes the simulated runtime's stream-ordering check (pbsim_cuda.h): no race between streams"""
+    import sim_engine
+    sim_engine.clear_races()
+    yield
+    sim_engine.assert_no_races()
+
+
 OPTION_DEFAULTS = {'h2d_pack': 0, 'tight_window': 1, 'profile': 1, 'direct_max': 160,
                    'chunk_tasks': 131072, 'pack_threads': 8, 'scratch_mb': 128, 'hbuf': 'auto'}
 
