@@ -105,6 +105,26 @@ int adapterEndDecisions(const pb200_end_batch_t *batches, int n_batches, int mat
  * none does (cmin[0] = INT32_MAX: 0/0 is NaN and never passes).  Pure host code. */
 int pb200TrimThresholdTable(double end_threshold, int32_t len, int32_t *cmin);
 
+/* Phase A of Porechop on the device: the adapter-set search (find_matching_adapter_sets, porechop.py:286-327, and
+ * NanoporeRead.align_adapter_set, nanopore_read.py:149-164).  Each batch is one cross product of read-end windows x adapter
+ * sequences (as in adapterAlignmentBatchMulti); the records stay on the device and a second kernel reduces them per adapter,
+ * so 8 bytes per adapter come back per submit instead of 36 per alignment:
+ *   best[a]  the value the reference leaves in best_start_score / best_end_score: 0.0, max'd (Python's max) with
+ *            float("%f" % fullAdapter%ID) of every alignment of adapter a in the batch.  A failed alignment (an empty
+ *            window included) contributes 0.0; a record with lenAdapter == 0 would be NaN, which never raises the maximum.
+ * The reduction is exact: the record with the largest 100.0*matchAdapter/lenAdapter in double gives the largest float, and
+ * the host formats that one with the reference's own snprintf("%f") / strtod chain.  Start windows x start sequences and end
+ * windows x end sequences go in one call as two batches.  A batch with n_seqs == 0 gives all 0.0; a batch with
+ * n_adapters == 0 is skipped (best is not touched).  batch.out may be NULL (records not copied back) or a buffer for the full
+ * records.  No preconditions beyond those of adapterAlignmentBatch: long windows (two-pass path) and scoring schemes of the
+ * generic int32 kernel are taken too. */
+typedef struct {
+    pb200_batch_t batch;   /* one cross product, as in adapterAlignmentBatchMulti; batch.out may be NULL */
+    double *best;          /* out: batch.n_adapters values */
+} pb200_search_batch_t;
+int adapterSetSearch(const pb200_search_batch_t *batches, int n_batches, int matchScore, int mismatchScore,
+                     int gapOpenScore, int gapExtensionScore);
+
 /* Same, with the bulk data already resident in device memory (d_seqs, d_seq_off, d_out are device pointers on
  * the current device; adapters/ad_off stay host pointers -- a few KB).  Cross-product mode only.
  * max_seq_len: length of the longest sequence, or -1 to let the library compute it on the device.
@@ -116,7 +136,7 @@ int pb200TrimThresholdTable(double end_threshold, int32_t len, int32_t *cmin);
  * Engine calls are ordered among themselves whatever their streams: every later call of this library, on any stream or
  * thread, waits for this one's queued work before it touches the engine's buffers.  Deferred errors (a traceback that left
  * its window) stay in a status word until pb200Synchronize reports and clears them; later calls that check the word
- * (adapterMiddleScanDevice and the host-buffer calls) report them too. */
+ * (adapterMiddleScanDevice and the host-buffer calls, adapterSetSearch included) report them too. */
 int adapterAlignmentBatchDevice(const uint8_t *d_seqs, const int64_t *d_seq_off, int64_t n_seqs,
                                 int64_t total_seq_bytes, int64_t max_seq_len, const uint8_t *adapters,
                                 const int32_t *ad_off, int32_t n_adapters, int matchScore, int mismatchScore,

@@ -55,6 +55,15 @@ class EndBatchDesc(Structure):
 
 C_LIB.adapterEndDecisions.argtypes = [POINTER(EndBatchDesc), c_int, c_int, c_int, c_int, c_int]
 C_LIB.adapterEndDecisions.restype = c_int
+
+
+class SearchBatchDesc(Structure):
+    """pb200_search_batch_t (include/porechop_b200.h)"""
+    _fields_ = [('batch', BatchDesc), ('best', c_void_p)]
+
+
+C_LIB.adapterSetSearch.argtypes = [POINTER(SearchBatchDesc), c_int, c_int, c_int, c_int, c_int]
+C_LIB.adapterSetSearch.restype = c_int
 C_LIB.pb200TrimThresholdTable.argtypes = [c_double, c_int32, c_void_p]
 C_LIB.pb200TrimThresholdTable.restype = c_int
 C_LIB.adapterAlignmentBatchMulti.argtypes = [POINTER(BatchDesc), c_int, c_int, c_int, c_int, c_int]
@@ -90,7 +99,8 @@ C_LIB.pb200PackNibbles.argtypes = [c_void_p, c_int64, c_void_p, c_int]
 C_LIB.pb200PackNibbles.restype = c_int
 
 EXPORTED_SYMBOLS = ['adapterAlignment', 'freeCString', 'adapterAlignmentBatch', 'adapterAlignmentBatchMulti',
-                    'adapterAlignmentBatchDevice', 'adapterEndDecisions', 'pb200TrimThresholdTable', 'adapterMiddleScan',
+                    'adapterAlignmentBatchDevice', 'adapterEndDecisions', 'pb200TrimThresholdTable', 'adapterSetSearch',
+                    'adapterMiddleScan',
                     'adapterMiddleScanDevice', 'pb200MiddleThresholdTable',
                     'pb200FormatRecord', 'pb200DeviceCount', 'pb200SetDevice', 'pb200Synchronize', 'pb200LastError',
                     'pb200KernelLaunches', 'pb200TimingEnable', 'pb200TimingRead', 'pb200TimingReadKinds', 'pb200SetOption',
@@ -250,6 +260,36 @@ def adapter_end_decisions(batches, scoring_scheme_vals, end_size, extra_trim_siz
     ma, mi, go, ge = [int(x) for x in scoring_scheme_vals]
     _check(C_LIB.adapterEndDecisions(descs, len(batches), ma, mi, go, ge))
     return outs
+
+
+def adapter_set_search(batches, scoring_scheme_vals):
+    """
+    Phase A on the device (adapterSetSearch): `batches` is a list of (seq_buf, seq_off, ad_buf, ad_off) or
+    (seq_buf, seq_off, ad_buf, ad_off, out) tuples with the array conventions of adapter_alignment_batch (`out`: an
+    int32[n_seqs * n_adapters, 9] array that receives the records too).  Returns one float64[n_adapters] per batch: the
+    best full-adapter identity of each adapter over the batch's windows, starting from 0.0, exactly as the reference's
+    best_start_score / best_end_score.
+    """
+    descs = (SearchBatchDesc * max(len(batches), 1))()
+    keep, bests = [], []
+    for k, b in enumerate(batches):
+        seq_buf = np.ascontiguousarray(b[0], dtype=np.uint8)
+        seq_off = np.ascontiguousarray(b[1], dtype=np.int64)
+        ad_buf = np.ascontiguousarray(b[2], dtype=np.uint8)
+        ad_off = np.ascontiguousarray(b[3], dtype=np.int32)
+        n_seqs, n_ad = len(seq_off) - 1, len(ad_off) - 1
+        out = b[4] if len(b) > 4 else None
+        if out is not None:
+            assert out.dtype == np.int32 and out.size == n_seqs * n_ad * RECORD_INTS and out.flags.c_contiguous
+        best = np.zeros(n_ad)
+        keep.append((seq_buf, seq_off, ad_buf, ad_off, out))
+        bests.append(best)
+        descs[k] = SearchBatchDesc(BatchDesc(seq_buf.ctypes.data, seq_off.ctypes.data, n_seqs, ad_buf.ctypes.data,
+                                             ad_off.ctypes.data, n_ad, out.ctypes.data if out is not None else None),
+                                   best.ctypes.data)
+    ma, mi, go, ge = [int(x) for x in scoring_scheme_vals]
+    _check(C_LIB.adapterSetSearch(descs, len(batches), ma, mi, go, ge))
+    return bests
 
 
 def trim_threshold_table(end_threshold, length):

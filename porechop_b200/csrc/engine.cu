@@ -191,6 +191,10 @@ struct Engine {
     // middle-adapter scan (adapterMiddleScan*): the resident segment -- codes (masked in place), offsets, records, next adapter
     // per read, hit slots, two active lists, threshold table, append counter + longest appended read
     DevBuf mid_codes, mid_off, mid_rec, mid_next_ad, mid_hits, mid_active[2], mid_cmin, mid_ctr;
+    // adapter-set search (adapterSetSearch): NSTAGE slices of search_cols u64 keys, one per stage, so that stages running at
+    // once never share an accumulator; a batch owns the columns [search_col, search_col + n_adapters) of every slice
+    DevBuf search_acc;
+    int64_t search_cols = 0;
     std::shared_ptr<void> packer;        // Packer (below): the thread that plans and packs chunks ahead of the submit loop
     // Ordering between calls: every entry point uses the stage buffers above (st[0]'s trace scratch, tasks, codes, status word),
     // whatever stream it runs on.  A call that returns with work still queued (adapterAlignmentBatchDevice) records `last` on
@@ -829,6 +833,9 @@ struct CrossJob {
     // middle scan (adapterMiddleScan): codes, offsets and records go to the segment's resident buffers instead of the stage's,
     // and middle_decide_kernel runs round 0 on each chunk; nothing is copied back
     const MiddleSeg *mid = nullptr;
+    // adapter-set search (adapterSetSearch): search_best_kernel reduces each chunk's records into the batch's columns of the
+    // stage's accumulator slice (Engine::search_acc); -1 = not a search batch
+    int64_t search_col = -1;
 };
 
 // The first chunks of a submit ramp up (1/8, 1/4, 1/2 of chunk_tasks): the pipeline's fill -- pack + H2D of chunk 0 before
@@ -1073,6 +1080,17 @@ int run_cross_jobs(Engine &E, std::vector<CrossJob> &jobs, int ma, int mi, int g
             if (a.top2)
                 CK(cudaMemcpyAsync(D.top2 + (size_t)s0 * 6, S.dec_top2.p, (size_t)cnt * 6 * 4, cudaMemcpyDeviceToHost, stream));
         }
+        if (J.search_col >= 0) {
+            unsigned long long *best = E.search_acc.as<unsigned long long>() + (size_t)(&S - E.st) * E.search_cols + J.search_col;
+            // one u64 per adapter in shared memory while that fits the default 48 KB of a block
+            const size_t smem_bytes = (size_t)J.n_adapters * 8;
+            const int use_smem = smem_bytes <= 48 * 1024 ? 1 : 0;
+            const int64_t blocks = std::max<int64_t>(1, std::min<int64_t>((cnt * J.n_adapters + 4095) / 4096, (int64_t)E.sm_count * 2));
+            search_best_kernel<<<(unsigned)blocks, 256, use_smem ? smem_bytes : 0, stream>>>(static_cast<const int32_t *>(S.out.as<int32_t>()),
+                                                                                 cnt, J.n_adapters, best, use_smem);
+            g_launches++;
+            CK(cudaGetLastError());
+        }
         if (J.out) {
             NvtxRange r("pb200:d2h");
             CK(cudaMemcpyAsync(J.out + (size_t)s0 * J.n_adapters * PB_REC, S.out.p, (size_t)cnt * J.n_adapters * PB_REC * 4,
@@ -1288,11 +1306,14 @@ int batch_host_multi(const pb200_batch_t *batches, int n_batches, int ma, int mi
 
 // float("%f" % (100.0*c/l)) exactly as the reference chain produces it: std::to_string(double) = sprintf("%f")
 // (porechop/src/alignment.cpp:113-121), then Python's float() = strtod (nanopore_read.py:488-489)
-double percent_exact(int32_t c, int32_t l) {
-    char buf[64];
-    volatile double cd = (double)c, ld = (double)l;
-    snprintf(buf, sizeof buf, "%f", 100.0 * cd / ld);
+double printed_exact(double d) {
+    char buf[512];                    // "%f" of any double up to 100.0 needs a few bytes; DBL_MAX would need 317
+    snprintf(buf, sizeof buf, "%f", d);
     return strtod(buf, nullptr);
+}
+double percent_exact(int32_t c, int32_t l) {
+    volatile double cd = (double)c, ld = (double)l;
+    return printed_exact(100.0 * cd / ld);
 }
 // inclusive = false: the end-trim test (value > thr); true: the middle-hit test (value >= thr)
 void threshold_table(double thr, int32_t len, bool inclusive, int32_t *cmin) {
@@ -1382,6 +1403,62 @@ int batch_end_decisions(const pb200_end_batch_t *batches, int n_batches, int ma,
     }
     CK(cudaStreamSynchronize(s0));               // tables are in place before any stage's stream uses them
     return run_cross_jobs(E, jobs, ma, mi, go, ge);
+}
+
+// Phase A on the device: every batch's records are max-reduced per adapter column (search_best_kernel) on the stage that made
+// them, into that stage's own accumulator slice; after the final drain the host takes the maximum over the slices and turns
+// the key back into float("%f" % d).
+int batch_search(const pb200_search_batch_t *batches, int n_batches, int ma, int mi, int go, int ge) {
+    if (n_batches < 0 || (n_batches > 0 && !batches)) return fail(PB200_ERR_ARG, "bad batch list");
+    load_env_options();
+    std::vector<CrossJob> jobs;
+    std::vector<double *> bests;
+    int64_t cols = 0;
+    for (int b = 0; b < n_batches; ++b) {
+        const pb200_batch_t &B = batches[b].batch;
+        if (B.n_seqs < 0 || B.n_adapters < 0) return fail(PB200_ERR_ARG, "negative count");
+        if (B.n_adapters == 0) continue;
+        double *best = batches[b].best;
+        if (!best) return fail(PB200_ERR_ARG, "NULL pointer");
+        if (B.n_seqs == 0) continue;
+        if (!B.seq_off || !B.ad_off) return fail(PB200_ERR_ARG, "NULL pointer");
+        if (int rc = validate_args(B.seqs, B.seq_off, B.n_seqs, B.adapters, B.ad_off, B.n_adapters, nullptr, nullptr,
+                                   B.n_seqs * (int64_t)B.n_adapters, true)) return rc;
+        CrossJob J{B.seqs, B.seq_off, B.n_seqs, B.adapters, B.ad_off, B.n_adapters, B.out};
+        J.search_col = cols;
+        cols += B.n_adapters;
+        jobs.push_back(std::move(J));
+        bests.push_back(best);
+    }
+    // every batch that has adapters starts from the reference's 0.0 (a batch without sequences keeps it)
+    for (int b = 0; b < n_batches; ++b)
+        if (batches[b].batch.n_adapters > 0) std::fill(batches[b].best, batches[b].best + batches[b].batch.n_adapters, 0.0);
+    if (jobs.empty()) return 0;
+    Engine *Ep = nullptr;
+    if (int rc = get_engine(&Ep)) return rc;
+    Engine &E = *Ep;
+    std::lock_guard<std::mutex> lk(E.mu);
+    if (int rc = E.init()) return rc;
+    if (int rc = order_stages_after_last(E)) return rc;
+    if (int rc = E.search_acc.ensure((size_t)NSTAGE * cols * 8)) return rc;
+    E.search_cols = cols;
+    for (int i = 0; i < NSTAGE; ++i)             // each slice is zeroed on the stream of the only stage that reduces into it
+        CK(cudaMemsetAsync(E.search_acc.as<unsigned long long>() + (size_t)i * cols, 0, (size_t)cols * 8, E.st[i].stream));
+    if (int rc = run_cross_jobs(E, jobs, ma, mi, go, ge)) return rc;
+    // run_cross_jobs drained every stage: the slices are final
+    std::vector<unsigned long long> keys((size_t)NSTAGE * cols);
+    CK(cudaMemcpyAsync(keys.data(), E.search_acc.p, keys.size() * 8, cudaMemcpyDeviceToHost, E.st[0].stream));
+    CK(cudaStreamSynchronize(E.st[0].stream));
+    for (size_t j = 0; j < jobs.size(); ++j) {
+        for (int32_t a = 0; a < jobs[j].n_adapters; ++a) {
+            unsigned long long k = 0;
+            for (int i = 0; i < NSTAGE; ++i) k = std::max(k, keys[(size_t)i * cols + jobs[j].search_col + a]);
+            double d;
+            memcpy(&d, &k, sizeof d);
+            bests[j][a] = printed_exact(d);
+        }
+    }
+    return 0;
 }
 
 // longest sequence of a device-resident batch (S.misc must hold 64 bytes)
@@ -1775,6 +1852,11 @@ int adapterAlignmentBatchMulti(const pb200_batch_t *batches, int n_batches, int 
 int adapterEndDecisions(const pb200_end_batch_t *batches, int n_batches, int ma, int mi, int go, int ge) {
     g_err.clear();
     return batch_end_decisions(batches, n_batches, ma, mi, go, ge);
+}
+
+int adapterSetSearch(const pb200_search_batch_t *batches, int n_batches, int ma, int mi, int go, int ge) {
+    g_err.clear();
+    return batch_search(batches, n_batches, ma, mi, go, ge);
 }
 
 int pb200TrimThresholdTable(double end_threshold, int32_t len, int32_t *cmin) {

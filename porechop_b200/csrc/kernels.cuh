@@ -7,6 +7,7 @@
 //   score_kernel<G,R,P>  streaming score-only overlap DP with exact scout (long reads), dynamic slot refill
 //   window_tasks_kernel  end cells of the score pass -> bounded-window tasks for trace_kernel
 //   decide_kernel        records -> per-read end-trim amounts + barcode score pairs (decisions stay on the device)
+//   search_best_kernel   records -> per-adapter best full-adapter identity of the adapter-set search (Phase A)
 //   middle_decide_kernel one round of the middle-adapter scan: first hit per active read, masking, next active list
 //   generic_kernel       int32 thread-serial fallback for scoring schemes / adapters outside the int16 domain
 //
@@ -14,6 +15,7 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <string.h>
 #include "dp_core.cuh"
 
 namespace pb {
@@ -812,6 +814,55 @@ __global__ void decide_kernel(const DecideArgs a, int *__restrict__ status) {
         }
     }
     if (ovf) atomicOr(status, 2);
+}
+
+// ---------------------------------------------------------------------------------------------------
+// search_best_kernel: records of one chunk (n reads x n_adapters, read-major, still in L2 from the DP kernels) -> per adapter
+// the largest full-adapter identity, max-reduced into `best` (the stage's accumulator columns of the batch).  The key of a
+// record is the bit pattern of d = 100.0 * c / l in IEEE double: 100 * c is exact and the division rounds to nearest, so d
+// is non-decreasing in c / l, and so is float("%f" % d) -- the largest key is the record with the largest Python float, and
+// a non-negative double's bits order like its value.  Records with l == 0 (failed alignments, empty windows) are skipped;
+// 0 is the key of +0.0, the reference's starting score.  Keys are reduced in shared memory first (one u64 per adapter,
+// use_smem = 1), then with one global atomic per adapter per block; use_smem = 0 (too many adapters for a block) goes
+// straight to `best`.  Plain arguments, no argument struct: `records` is only read, `best` is only updated atomically.
+__device__ __forceinline__ unsigned long long percent_key(int32_t c, int32_t l) {
+    const double d = 100.0 * (double)c / (double)l;
+#if defined(__CUDA_ARCH__)
+    return (unsigned long long)__double_as_longlong(d);
+#else
+    unsigned long long k;
+    memcpy(&k, &d, sizeof k);
+    return k;
+#endif
+}
+__global__ void search_best_kernel(const int32_t *__restrict__ records, int64_t n, int32_t n_adapters, unsigned long long *best,
+                                   int use_smem) {
+    extern __shared__ uint32_t smem[];
+    unsigned long long *acc = use_smem ? reinterpret_cast<unsigned long long *>(smem) : best;
+    if (use_smem) {
+        for (int k = threadIdx.x; k < n_adapters; k += blockDim.x) acc[k] = 0ull;
+        __syncthreads();
+    }
+    const int64_t total = n * n_adapters;
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    int32_t col = (int32_t)(i % n_adapters);
+    const int32_t step = (int32_t)(stride % n_adapters);
+    for (; i < total; i += stride) {
+        const int32_t *r = records + (size_t)i * PB_REC;
+        const int32_t l = r[8];
+        if (l > 0) {
+            const unsigned long long key = percent_key(r[7], l);
+            if (key > acc[col]) atomicMax(&acc[col], key);       // the plain read only skips atomics that cannot raise it
+        }
+        col += step;
+        if (col >= n_adapters) col -= n_adapters;
+    }
+    if (use_smem) {
+        __syncthreads();
+        for (int k = threadIdx.x; k < n_adapters; k += blockDim.x)
+            if (acc[k]) atomicMax(&best[k], acc[k]);
+    }
 }
 
 // ---------------------------------------------------------------------------------------------------

@@ -21,7 +21,8 @@ buffers end to end:
   middle_trim_ranges(...)    hits -> the ranges the reference adds to `middle_trim_positions`
   emit(...)                  get_fastq / get_fasta of every read (split parts, numbering, --discard_middle,
                              --min_split_read_size, RNA T->U) as one bytes object, assembled with vectorised scatters
-  search_adapter_sets(...)   Phase A: best start / end identity of every adapter set over the check reads' windows
+  search_adapter_sets(...)   Phase A: best start / end identity of every adapter set over the check reads' windows --
+                             or, with PB200_DEVICE_SEARCH=1, one adapterSetSearch call that reduces them on the device
   trim_fastq(...)            all of the above for a fixed list of adapter sets: what `porechop -i x.fastq -o y.fastq`
                              writes once Phase A has chosen the sets
   call_barcodes(...)         determine_barcode (nanopore_read.py:399-470) on score matrices: best / second-best
@@ -559,25 +560,42 @@ def _assemble(batch, names, fmt, read, s0, slen, q0, qlen, n0, nlen, rec_len):
 
 
 # ---------------------------------------------------------------------------------------------------------------
-def search_adapter_sets(batch, adapter_sets, scoring_scheme_vals, check_reads=10000, end_size=150):
+# Phase A on the device (include/porechop_b200.h adapterSetSearch): the records of the search are reduced to one best score
+# per adapter sequence before anything is copied back -- 8 bytes per sequence instead of 36 per (window, sequence).  Off by
+# default.
+DEVICE_SEARCH = os.environ.get('PB200_DEVICE_SEARCH', '0') == '1'
+
+
+def search_adapter_sets(batch, adapter_sets, scoring_scheme_vals, check_reads=10000, end_size=150, device=None):
     """Phase A (porechop.py:286-327, nanopore_read.py:149-164) on a FastqBatch: the best full-adapter identity of every
     set's start / end sequence over the end windows of the first `check_reads` reads.  adapter_sets as for trim_fastq.
     Returns (best_start_score[k], best_end_score[k]) (0.0 where a set has no such sequence); the caller applies the
-    reference's policy on top (`>= adapter_threshold`, porechop.py:327; 1D^2 fix-up, barcode kit choice)."""
+    reference's policy on top (`>= adapter_threshold`, porechop.py:327; 1D^2 fix-up, barcode kit choice).
+    device (default: the module switch DEVICE_SEARCH): one adapterSetSearch call with both batches instead; the same
+    scores come back."""
+    if device is None:
+        device = DEVICE_SEARCH
     sets = _norm_sets(adapter_sets)
     k = min(int(check_reads), len(batch))
     best_s, best_e = np.zeros(len(sets)), np.zeros(len(sets))
     if k == 0:
         return best_s, best_e
     (sbuf, soff), (ebuf, eoff) = end_windows(batch.seq, batch.seq_off[:k + 1], end_size)
+    searched = []
     for which, buf, off, best in ((1, sbuf, soff, best_s), (2, ebuf, eoff, best_e)):
         idx = [j for j, t in enumerate(sets) if t[which]]
         if not idx:
             continue
         abuf, aoff = W.pack_sequences([sets[j][which][1] for j in idx], offset_dtype=np.int32)
+        if device:
+            searched.append((idx, best, (buf, off, abuf, aoff)))
+            continue
         rec = W.adapter_alignment_batch(buf, off, abuf, aoff, scoring_scheme_vals)
         full, _, _, _ = scores_from_records(rec)
         best[idx] = np.maximum(full.reshape(k, len(idx)).max(axis=0), 0.0)
+    if searched:
+        for (idx, best, _), got in zip(searched, W.adapter_set_search([x[2] for x in searched], scoring_scheme_vals)):
+            best[idx] = got
     return best_s, best_e
 
 

@@ -15,7 +15,8 @@ reads of Phase A), so memory is bounded by the chunk size, not the file size.
 Opt-in device paths (environment, off by default; output bytes are the same): PB200_DEVICE_DECISIONS=1 runs the end-trim
 decisions on the device (adapterEndDecisions), PB200_DEVICE_MIDDLE=1 runs the whole middle-adapter scan there, masking
 rounds included (adapterMiddleScan; inputs it does not take -- e.g. adapters with other bases than A/C/G/T/U -- use the
-host rounds), PB200_CHECK_ALL_READS=1 runs Phase A over every read.
+host rounds), PB200_CHECK_ALL_READS=1 runs Phase A over every read, and PB200_DEVICE_SEARCH=1 reduces Phase A's records to
+one best score per adapter sequence on the device (adapterSetSearch) -- what makes checking every read cheap.
 
 Multi-GPU: launched with torchrun (one process per GPU) chunk c is handled by rank c % world on its own device; ranks
 write self-contained pieces and rank 0 stitches them in chunk order after a barrier -- no data-path collective

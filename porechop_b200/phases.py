@@ -44,12 +44,27 @@ def _cross(windows, adapter_seqs, scoring):
 
 
 # ----------------------------------------------------------------------------------------------------------------
-def align_adapter_sets(check_reads, adapter_sets, end_size, scoring_scheme_vals):
+def align_adapter_sets(check_reads, adapter_sets, end_size, scoring_scheme_vals, device=None):
     """Phase A: keep, per adapter set, the best full-adapter identity of its start / end sequence over the check
-    reads' end windows (reference: best_start_score / best_end_score updated read by read with max())."""
+    reads' end windows (reference: best_start_score / best_end_score updated read by read with max()).
+    device (default: fastq.DEVICE_SEARCH, PB200_DEVICE_SEARCH=1): one adapterSetSearch call reduces both batches on the
+    device and fills the same fields."""
     starts = [(k, s.start_sequence[1]) for k, s in enumerate(adapter_sets) if s.start_sequence]
     ends = [(k, s.end_sequence[1]) for k, s in enumerate(adapter_sets) if s.end_sequence]
     if not check_reads:
+        return
+    if device is None:
+        from .fastq import DEVICE_SEARCH as device
+    if device:
+        batches, fields = [], []
+        for lst, windows, field in ((starts, [r.seq[:end_size] for r in check_reads], 'best_start_score'),
+                                    (ends, [r.seq[-end_size:] for r in check_reads], 'best_end_score')):
+            if lst:
+                batches.append(_pack(windows, np.int64) + _pack([x[1] for x in lst], np.int32))
+                fields.append((lst, field))
+        for (lst, field), best in zip(fields, W.adapter_set_search(batches, scoring_scheme_vals)):
+            for (k, _), b in zip(lst, best):
+                setattr(adapter_sets[k], field, max(getattr(adapter_sets[k], field), float(b)))
         return
     if starts:
         full, _, _, _ = _cross([r.seq[:end_size] for r in check_reads], [x[1] for x in starts], scoring_scheme_vals)

@@ -5,11 +5,18 @@ metric (bench.py measures the alignment path itself); this is the tool for findi
 
     python tools/flat_pipeline_bench.py --reads 200000 --repeat 3
     python tools/flat_pipeline_bench.py --reads 200000 --middle both    # Phase C: host rounds vs adapterMiddleScan
+    python tools/flat_pipeline_bench.py --reads 200000 --search both    # Phase A over every read: host vs adapterSetSearch
 
 --middle host|device|both times Phase C with the host masking rounds (fastq.find_middle_hits' default) and / or the device
 scan (PB200_DEVICE_MIDDLE), alternating the two over the same FASTQ; it reports per path the `middle` seconds of trim_fastq,
 rounds, hit reads, hits and the bytes Phase C copies in each direction (counted from the shapes of the engine calls), the
 card and its power limit, and asserts that both paths write identical bytes.
+
+--search host|device|both times Phase A over every read (check_reads = number of reads, the 236 sequences of the 119 table
+sets, what PB200_CHECK_ALL_READS=1 does) with the record path (fastq.search_adapter_sets' default) and / or the device
+reduction (PB200_DEVICE_SEARCH), alternating the two over the same FASTQ; it reports per path the seconds of
+search_adapter_sets and the bytes it copies in each direction (counted from the shapes of the engine calls), the card and its
+power limit, and asserts that both paths return identical scores.
 """
 import argparse
 import json
@@ -138,14 +145,73 @@ def run_middle(n_reads, repeat, which, seed=20260923):
             'paths': res}
 
 
+def _phase_a_counter(W):
+    """wraps the engine calls of search_adapter_sets: bytes each way, from the shapes of what crosses the C-ABI"""
+    st = {'h2d_bytes': 0, 'd2h_bytes': 0}
+    orig_batch, orig_search = W.adapter_alignment_batch, W.adapter_set_search
+
+    def batch(seq_buf, seq_off, ad_buf, ad_off, scoring, pair_seq=None, pair_adapter=None, out=None):
+        r = orig_batch(seq_buf, seq_off, ad_buf, ad_off, scoring, pair_seq, pair_adapter, out)
+        st['h2d_bytes'] += seq_buf.nbytes + seq_off.nbytes + ad_buf.nbytes + ad_off.nbytes
+        st['d2h_bytes'] += r.nbytes
+        return r
+
+    def search(batches, scoring):
+        got = orig_search(batches, scoring)
+        for b, g in zip(batches, got):
+            st['h2d_bytes'] += sum(x.nbytes for x in b[:4])
+            st['d2h_bytes'] += 3 * g.nbytes                   # one u64 key per adapter in each of the engine's 3 stage slices
+        return got
+    return st, (batch, search), (orig_batch, orig_search)
+
+
+def run_search(n_reads, repeat, which, seed=20260923):
+    import numpy as np
+    from porechop_b200 import fastq, workloads as wl
+    data, _, _ = synthetic_fastq(n_reads, seed)
+    batch = fastq.parse_fastq(data)
+    sets = [(d['name'], d['start'] or None, d['end'] or None) for d in wl.load_adapter_sets()['sets']]
+    n_seqs = sum(bool(s) + bool(e) for _, s, e in sets)
+    paths = ['host', 'device'] if which == 'both' else [which]
+    res, scores = {p: None for p in paths}, {}
+    W = fastq.W
+    fastq.search_adapter_sets(batch, sets, wl.DEFAULT_SCORING, 1000)           # warm-up: plans, buffers, modules
+    fastq.search_adapter_sets(batch, sets, wl.DEFAULT_SCORING, 1000, device=True)
+    for _ in range(repeat):
+        for p in paths:                                       # alternated: the host's other work hits both alike
+            st, (b, s), orig = _phase_a_counter(W)
+            W.adapter_alignment_batch, W.adapter_set_search = b, s
+            try:
+                t0 = time.perf_counter()
+                got = fastq.search_adapter_sets(batch, sets, wl.DEFAULT_SCORING, len(batch), device=p == 'device')
+                sec = time.perf_counter() - t0
+            finally:
+                W.adapter_alignment_batch, W.adapter_set_search = orig
+            scores.setdefault(p, got)
+            assert all(np.array_equal(a, b) for a, b in zip(scores[p], got))
+            cur = {'phase_a_s': sec, 'h2d_bytes': st['h2d_bytes'], 'd2h_bytes': st['d2h_bytes']}
+            if res[p] is None or cur['phase_a_s'] < res[p]['phase_a_s']:
+                res[p] = cur
+    identical = all(all(np.array_equal(a, b) for a, b in zip(scores[paths[0]], scores[p])) for p in paths)
+    if len(paths) == 2:
+        assert identical, 'host and device adapter-set searches returned different scores'
+    return {'reads': n_reads, 'in_bytes': len(data), 'sequences': n_seqs, 'card': card(), 'repeat': repeat,
+            'identical_scores': identical, 'sets_found': int(sum(max(x, y) >= 90.0 for x, y in zip(*scores[paths[0]]))),
+            'paths': res}
+
+
 if __name__ == '__main__':
     ap = argparse.ArgumentParser()
     ap.add_argument('--reads', type=int, default=100000)
     ap.add_argument('--repeat', type=int, default=3)
     ap.add_argument('--middle', choices=['host', 'device', 'both'], default=None,
                     help='time Phase C with the host rounds, the device scan, or both alternately')
+    ap.add_argument('--search', choices=['host', 'device', 'both'], default=None,
+                    help='time Phase A over every read with the record path, the device reduction, or both alternately')
     a = ap.parse_args()
-    if a.middle:
+    if a.search:
+        print(json.dumps(run_search(a.reads, a.repeat, a.search)))
+    elif a.middle:
         print(json.dumps(run_middle(a.reads, a.repeat, a.middle)))
     else:
         print(json.dumps(run(a.reads, a.repeat)))

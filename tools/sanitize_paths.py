@@ -71,5 +71,18 @@ bad += 0 if ok else 1
 print('top2      %s' % ('ok' if ok else 'DIFFERENT'), flush=True)
 got = W.adapter_alignment_batch_multi([(sbuf, soff, a1, o1), (lbuf, loff, a2, o2)], wl.DEFAULT_SCORING)
 bad += 0 if np.array_equal(got[1], oracle_batch(lbuf, loff, a2, o2, wl.DEFAULT_SCORING)) else 1
+# adapter-set search (Phase A): the per-adapter maxima against the host reduction of the oracle's records, over 227 and 2
+# adapter columns, with long reads on the two-pass path and with many small chunks
+from porechop_b200.align import scores_from_records
+for opts in ({}, {'direct_max': 100, 'chunk_tasks': 200}):
+    def search():
+        batches = [(sbuf[:150 * 40], soff[:41], a3, o3), (lbuf, loff, a2, o2)]
+        got = W.adapter_set_search(batches, wl.DEFAULT_SCORING)
+        exp = []
+        for b, o, a, ao in batches:
+            full = scores_from_records(oracle_batch(b, o, a, ao, wl.DEFAULT_SCORING))[0].reshape(len(o) - 1, len(ao) - 1)
+            exp.append(np.maximum(full.max(axis=0), 0.0))
+        return np.concatenate(got), np.concatenate(exp)
+    run('search', opts, search)
 print('SANITIZE RUN COMPLETE, %d wrong' % bad, flush=True)
 sys.exit(1 if bad else 0)
