@@ -23,10 +23,9 @@ namespace pb {
 constexpr int PB_WARPS_PER_BLOCK = 4;
 // trace_kernel blocks per SM.  Groups of G <= 8 lanes: 6 (80 registers), which the default trace scratch and the shared
 // memory hold for end windows (the scratch of a warp grows with G: 128 MB holds 6 blocks per SM of G = 4 / 8 at 150 columns,
-// 5 of G = 16 / 32).  The end-trim classes then spill, but only values of the slot set-up, the final-column scout and the
-// traceback; the hot 4-step chunk stays spill-free and no longer (DESIGN.md section 4).  On an H100 80GB HBM3 at a 700 W
-// power limit the end-trim launches ran 2.9 % faster than at 5 blocks.  Wider groups keep 5 blocks (96 registers): a sixth
-// block would not fit their scratch.
+// 5 of G = 16 / 32).  Since the final-column scout runs inside the careful step (lane_step<.., FCOL>) the end-trim classes
+// spill at most 4 bytes (DESIGN.md section 4).  On an H100 80GB HBM3 at a 700 W power limit the end-trim launches ran 2.9 %
+// faster than at 5 blocks.  Wider groups keep 5 blocks (96 registers): a sixth block would not fit their scratch.
 #ifndef PB_TRACE_MIN_BLOCKS
 #define PB_TRACE_MIN_BLOCKS 6
 #endif
@@ -285,7 +284,9 @@ __device__ __forceinline__ void stage_columns(uint32_t *hbuf, int g, const uint8
 // by two lanes of the group, 9-int record per alignment.  Grid-stride over "warp slots" so the trace scratch is
 // bounded by the resident grid and stays in L2.
 // (Measured and removed: a score-only first pass + bounded trace window for 150-column windows, and shared-memory query
-// profiles for the substitution operands -- neither beat this single pass.)
+// profiles for the substitution operands -- neither beat this single pass.  Running the final columns as unrolled 4-step
+// chunks too (the general scout behind a warp vote, lanes past the end on the last staged column) made the end-trim launches
+// 27 % slower: 6.31-6.36 instead of 4.96-5.01 ms per step.)
 template <int G, int R, bool HBUF_SMEM>
 __global__ void __launch_bounds__(PB_WARPS_PER_BLOCK * 32, G <= 8 ? PB_TRACE_MIN_BLOCKS : PB_TRACE_MIN_BLOCKS_WIDE)
 trace_kernel(const TaskSrc ts, const uint8_t *__restrict__ seq,
@@ -361,9 +362,18 @@ trace_kernel(const TaskSrc ts, const uint8_t *__restrict__ seq,
         constexpr int TWARM = (G - 1 + PB_TCHUNK - 1) & ~(PB_TCHUNK - 1);
         int tfast = need_track ? (nmin - 1) : nmax;
         tfast = __reduce_min_sync(0xffffffffu, max(tfast, 0)) & ~(PB_TCHUNK - 1);
+#ifdef PB_EXPERIMENT_ALL_HOT   // (timing experiment only, wrong records: every chunk takes the hot path; tools/trace_phase_cost.py)
+#define PB_HOT_COL(j) max(min((j) - 1, nmax - 1), 0)       // stay inside the staged bases
+#else
+#define PB_HOT_COL(j) ((j) - 1)
+#endif
         for (int t0 = 0; t0 < T4; t0 += PB_TCHUNK) {
             uint4 acc[WPS];
+#ifdef PB_EXPERIMENT_ALL_HOT
+            if (true) {
+#else
             if (t0 >= TWARM && t0 < tfast) {
+#endif
                 uint32_t buf[PB_TCHUNK][WPS];
 #pragma unroll
                 for (int u = 0; u < PB_TCHUNK; ++u) {
@@ -371,7 +381,7 @@ trace_kernel(const TaskSrc ts, const uint8_t *__restrict__ seq,
                     uint32_t recvV = __shfl_up_sync(0xffffffffu, L.botV, 1, G);
                     if (g == 0) { recvS = sc.borderX2; recvV = sc.negb2; }
                     const int j = t0 + u - g + 1;
-                    lane_step<R, true, false>(L, recvS, recvV, hbuf[j - 1], sc, buf[u]);
+                    lane_step<R, true, false>(L, recvS, recvV, hbuf[PB_HOT_COL(j)], sc, buf[u]);
                     if (need_track) lane_track_lastrow<R>(L, j, sc);
                 }
 #pragma unroll
@@ -389,12 +399,21 @@ trace_kernel(const TaskSrc ts, const uint8_t *__restrict__ seq,
                     uint32_t tw[WPS];
 #pragma unroll
                     for (int w = 0; w < WPS; ++w) tw[w] = 0u;
-                    if (j >= 1 && j <= nmax) {
-                        uint32_t vr[R];
-                        lane_step<R, true, true>(L, recvS, recvV, hbuf[j - 1], sc, tw, vr);
-                        if (need_track) {
-                            if (j >= nmin) lane_track_general<R>(L, g, j, make_geom(nA, mA, G, R), make_geom(nB, mB, G, R), vr, sc);
-                            else lane_track_lastrow<R>(L, j, sc);
+                    // the final-column scout runs inside the step, row by row, and only in the steps in which some lane of the
+                    // warp is past the inner columns of a half (G steps per slot for uniform windows): no Vs registers kept
+                    const bool in = j >= 1 && j <= nmax;
+                    const bool fin = in && need_track && j >= nmin;
+                    const bool any_fin = !__all_sync(0xffffffffu, !fin);
+                    if (in) {
+                        if (any_fin) {
+                            FinalCol fc;
+                            fc.mask = fin ? ((j == nA ? 1 : 0) | (j == nB ? 2 : 0)) : 0;
+                            fc.i0[0] = g * R + 1 - (G * R - mA); fc.i0[1] = g * R + 1 - (G * R - mB);
+                            lane_step<R, true, false, false, true>(L, recvS, recvV, hbuf[j - 1], sc, tw, nullptr, nullptr, &fc);
+                            if (need_track) lane_track_general<R, false>(L, g, j, make_geom(nA, mA, G, R), make_geom(nB, mB, G, R), nullptr, sc);
+                        } else {
+                            lane_step<R, true, false>(L, recvS, recvV, hbuf[j - 1], sc, tw);
+                            if (need_track) lane_track_lastrow<R>(L, j, sc);
                         }
                     }
 #pragma unroll
@@ -424,6 +443,9 @@ trace_kernel(const TaskSrc ts, const uint8_t *__restrict__ seq,
                 } else {
                     end = scout_combine(cand + h * 32 + grp * G, G, gh);
                 }
+#ifdef PB_EXPERIMENT_ALL_HOT   // the scout saw columns past the end: keep the traceback inside the matrix
+                end.j = min(end.j, tk.n); end.i = min(end.i, tk.m);
+#endif
                 // cursor over the slot's trace: incremental addresses (lane of the row, row within the lane, step index) instead
                 // of a division per path step; one 128-bit load serves up to PB_TCHUNK consecutive steps of a lane
                 struct Cursor {
