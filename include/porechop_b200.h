@@ -168,6 +168,47 @@ int adapterMiddleScanDevice(const uint8_t *d_seqs, const int64_t *d_seq_off, int
                             int matchScore, int mismatchScore, int gapOpenScore, int gapExtensionScore,
                             double middle_threshold, int32_t *n_hits, int32_t *hits, int64_t hits_cap, int64_t *n_total,
                             void *stream);
+/* Phase B and Phase C of Porechop on whole reads in one call: the semantics of adapterEndDecisions over the windows
+ * seq[:end_size] / seq[-end_size:] of every read, followed by adapterMiddleScan over seq[start_trim : len - end_trim] (Python's
+ * slice: an end position below 0 counts from the end of the read again; an untrimmed read is the whole read).  The windows
+ * are cut, the trims decided and turned into the trimmed reads, and the trimmed reads encoded and masked on the device, so
+ * the read bytes cross PCIe once (host variant) or not at all (device variant), and 4 bytes per read per side, the score
+ * outputs and the hits come back.
+ *   start / end    one side of Phase B (find_start_trim / find_end_trim): adapters, score columns and outputs with the
+ *                  meaning of the pb200_end_batch_t fields of the same names; n_adapters = 0: the side is not searched, its
+ *                  trims are 0 (and top2, if given, the "no column" entries)
+ *   mid_*          the middle adapters in the reference's order; n_mid_adapters = 0: no Phase C (--no_split), and n_hits /
+ *                  hits / n_total may then be NULL (written as zero / empty when given)
+ *   n_hits, hits   as adapterMiddleScan, in trimmed-read coordinates; on PB200_ERR_SPACE the trims, the score outputs,
+ *                  n_hits and *n_total are valid
+ * Preconditions, checked before the device is touched (PB200_ERR_ARG otherwise): those of adapterEndDecisions for each side
+ * and of adapterMiddleScan for the middle adapters, end_size >= 1, and every adapter of every side served by the int16
+ * kernels with a finite window bound (both gap scores negative; no generic-class scheme). */
+typedef struct {
+    const uint8_t *adapters; const int32_t *ad_off; int32_t n_adapters;   /* 0 = side not searched, trims = 0 */
+    const int32_t *score_cols; int32_t n_score_cols;                      /* as pb200_end_batch_t */
+    int32_t *trim;                                                        /* out: n_seqs */
+    uint16_t *score_pairs;                                                /* out: as pb200_end_batch_t (may be NULL) */
+    int32_t *top2;                                                        /* out: as pb200_end_batch_t (may be NULL) */
+} pb200_trim_side_t;
+typedef struct {
+    int32_t end_size, extra_trim_size, min_trim_size;   /* --end_size (>= 1), --extra_end_trim, --min_trim_size */
+    double end_threshold;                               /* --end_threshold (>= 0) */
+    pb200_trim_side_t start, end;
+    const uint8_t *mid_adapters; const int32_t *mid_ad_off; int32_t n_mid_adapters;   /* 0 = no Phase C */
+    double middle_threshold;                            /* --middle_threshold (> 0 when there are middle adapters) */
+    int32_t *n_hits; int32_t *hits; int64_t hits_cap; int64_t *n_total;   /* outputs, as adapterMiddleScan */
+} pb200_trim_args_t;
+int adapterTrimReads(const uint8_t *seqs, const int64_t *seq_off, int64_t n_seqs, const pb200_trim_args_t *args,
+                     int matchScore, int mismatchScore, int gapOpenScore, int gapExtensionScore);
+/* Same, with seqs / seq_off in device memory (conventions of adapterMiddleScanDevice: max_seq_len = longest read or -1; the
+ * caller's buffers are only read; the work runs on `stream` -- NULL: the library's own stream after the legacy default
+ * stream -- after the work earlier calls of this library left queued on any stream; the outputs are host buffers, so the
+ * call returns only after they are written, and reports a deferred error an earlier device-resident call left in the status
+ * word). */
+int adapterTrimReadsDevice(const uint8_t *d_seqs, const int64_t *d_seq_off, int64_t n_seqs, int64_t total_seq_bytes,
+                           int64_t max_seq_len, const pb200_trim_args_t *args, int matchScore, int mismatchScore,
+                           int gapOpenScore, int gapExtensionScore, void *stream);
 /* cmin[l], l = 0 .. len-1: the smallest c with float("%f" % (100.0*c/l)) >= middle_threshold, or l+1 if none does
  * (cmin[0] = INT32_MAX).  The ">=" sibling of pb200TrimThresholdTable.  Pure host code; middle_threshold must be > 0. */
 int pb200MiddleThresholdTable(double middle_threshold, int32_t len, int32_t *cmin);

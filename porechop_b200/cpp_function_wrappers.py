@@ -12,7 +12,7 @@ There is no CPU fallback: if cpp_functions.so is missing the import exits like t
 
 import os
 import sys
-from ctypes import CDLL, POINTER, Structure, byref, c_char_p, c_double, c_int, c_int32, c_int64, c_longlong, c_void_p, cast, \
+from ctypes import CDLL, POINTER, Structure, addressof, byref, c_char_p, c_double, c_int, c_int32, c_int64, c_longlong, c_void_p, cast, \
     create_string_buffer
 
 import numpy as np
@@ -77,6 +77,27 @@ C_LIB.adapterMiddleScan.restype = c_int
 C_LIB.adapterMiddleScanDevice.argtypes = [c_void_p, c_void_p, c_int64, c_int64, c_int64, c_void_p, c_void_p, c_int32, c_int,
                                           c_int, c_int, c_int, c_double, c_void_p, c_void_p, c_int64, c_void_p, c_void_p]
 C_LIB.adapterMiddleScanDevice.restype = c_int
+
+
+class TrimSideDesc(Structure):
+    """pb200_trim_side_t (include/porechop_b200.h)"""
+    _fields_ = [('adapters', c_void_p), ('ad_off', c_void_p), ('n_adapters', c_int32), ('score_cols', c_void_p),
+                ('n_score_cols', c_int32), ('trim', c_void_p), ('score_pairs', c_void_p), ('top2', c_void_p)]
+
+
+class TrimArgsDesc(Structure):
+    """pb200_trim_args_t (include/porechop_b200.h)"""
+    _fields_ = [('end_size', c_int32), ('extra_trim_size', c_int32), ('min_trim_size', c_int32), ('end_threshold', c_double),
+                ('start', TrimSideDesc), ('end', TrimSideDesc), ('mid_adapters', c_void_p), ('mid_ad_off', c_void_p),
+                ('n_mid_adapters', c_int32), ('middle_threshold', c_double), ('n_hits', c_void_p), ('hits', c_void_p),
+                ('hits_cap', c_int64), ('n_total', c_void_p)]
+
+
+C_LIB.adapterTrimReads.argtypes = [c_void_p, c_void_p, c_int64, POINTER(TrimArgsDesc), c_int, c_int, c_int, c_int]
+C_LIB.adapterTrimReads.restype = c_int
+C_LIB.adapterTrimReadsDevice.argtypes = [c_void_p, c_void_p, c_int64, c_int64, c_int64, POINTER(TrimArgsDesc), c_int, c_int,
+                                         c_int, c_int, c_void_p]
+C_LIB.adapterTrimReadsDevice.restype = c_int
 C_LIB.pb200MiddleThresholdTable.argtypes = [c_double, c_int32, c_void_p]
 C_LIB.pb200MiddleThresholdTable.restype = c_int
 C_LIB.pb200FormatRecord.argtypes = [c_void_p, c_char_p, c_int]
@@ -101,7 +122,7 @@ C_LIB.pb200PackNibbles.restype = c_int
 EXPORTED_SYMBOLS = ['adapterAlignment', 'freeCString', 'adapterAlignmentBatch', 'adapterAlignmentBatchMulti',
                     'adapterAlignmentBatchDevice', 'adapterEndDecisions', 'pb200TrimThresholdTable', 'adapterSetSearch',
                     'adapterMiddleScan',
-                    'adapterMiddleScanDevice', 'pb200MiddleThresholdTable',
+                    'adapterMiddleScanDevice', 'pb200MiddleThresholdTable', 'adapterTrimReads', 'adapterTrimReadsDevice',
                     'pb200FormatRecord', 'pb200DeviceCount', 'pb200SetDevice', 'pb200Synchronize', 'pb200LastError',
                     'pb200KernelLaunches', 'pb200TimingEnable', 'pb200TimingRead', 'pb200TimingReadKinds', 'pb200SetOption',
                     'pb200GetOption', 'pb200HostBuffer', 'pb200PackNibbles']
@@ -357,6 +378,80 @@ def adapter_middle_scan_device(d_seqs_ptr, d_seq_off_ptr, n_seqs, total_seq_byte
     return _middle_scan(lambda nh, h, cap, total: C_LIB.adapterMiddleScanDevice(
         c_void_p(d_seqs_ptr), c_void_p(d_seq_off_ptr), n_seqs, total_seq_bytes, max_seq_len, _ptr(ad_buf), _ptr(ad_off),
         len(ad_off) - 1, ma, mi, go, ge, float(middle_threshold), nh, h, cap, total, c_void_p(stream_ptr)), int(n_seqs))
+
+
+def _trim_reads(call, n_seqs, start, end, middle, end_size, extra_trim_size, end_threshold, min_trim_size, middle_threshold,
+                want_top2):
+    """adapterTrimReads(Device) with caller-owned outputs: builds pb200_trim_args_t, starts with room for 2n + 1024 hits and
+    retries once with exactly *n_total when the engine answers PB200_ERR_SPACE (as _middle_scan)."""
+    keep, sides, outs = [], [], []
+    for ad_buf, ad_off, cols in (start, end):
+        ad_buf = np.ascontiguousarray(ad_buf, dtype=np.uint8)
+        ad_off = np.ascontiguousarray(ad_off, dtype=np.int32)
+        cols = np.ascontiguousarray(cols if cols is not None else [], dtype=np.int32)
+        trim = np.zeros(n_seqs, dtype=np.int32)
+        if want_top2:
+            scores = np.tile(np.array([-1, 0, 1], dtype=np.int32), (n_seqs, 2))
+        else:
+            scores = np.zeros((n_seqs, len(cols), 2), dtype=np.uint16)
+        keep.append((ad_buf, ad_off, cols))
+        outs.append((trim, scores))
+        sides.append(TrimSideDesc(ad_buf.ctypes.data, ad_off.ctypes.data, len(ad_off) - 1, cols.ctypes.data if len(cols) else None,
+                                  len(cols), trim.ctypes.data, scores.ctypes.data if (len(cols) and not want_top2) else None,
+                                  scores.ctypes.data if (len(cols) and want_top2) else None))
+    if middle is not None:
+        mid_buf = np.ascontiguousarray(middle[0], dtype=np.uint8)
+        mid_off = np.ascontiguousarray(middle[1], dtype=np.int32)
+    else:
+        mid_buf, mid_off = np.zeros(0, dtype=np.uint8), np.zeros(1, dtype=np.int32)
+    n_hits = np.zeros(n_seqs, dtype=np.int32)
+    total = c_int64(0)
+    cap = 2 * n_seqs + 1024
+    for _ in range(2):
+        hits = np.empty((cap, HIT_INTS), dtype=np.int32)
+        args = TrimArgsDesc(int(end_size), int(extra_trim_size), int(min_trim_size), float(end_threshold), sides[0], sides[1],
+                            mid_buf.ctypes.data, mid_off.ctypes.data, len(mid_off) - 1, float(middle_threshold),
+                            n_hits.ctypes.data, hits.ctypes.data, cap, addressof(total))
+        rc = call(byref(args))
+        if rc == ERR_SPACE and total.value > cap:
+            cap = total.value
+            continue
+        break
+    _check(rc)
+    (st, ss), (et, es) = outs
+    return st, et, ss, es, n_hits, hits[:total.value]
+
+
+def adapter_trim_reads(seq_buf, seq_off, start, end, middle, scoring_scheme_vals, end_size, extra_trim_size, end_threshold,
+                       min_trim_size, middle_threshold=85.0, want_top2=False):
+    """
+    Porechop's Phase B and Phase C on whole reads in one engine call (adapterTrimReads): the end windows are cut, the trims
+    decided, and the trimmed reads scanned for middle adapters on the device; the reads are uploaded once.
+    seq_buf / seq_off: the reads (uint8, int64[n+1]).  start / end: (ad_buf, ad_off, score_cols) of find_start_trim /
+    find_end_trim (ad_off int32; no adapters = the side is not searched); middle: (ad_buf, ad_off) of the middle adapters in
+    the reference's order, or None (--no_split).
+    Returns (start_trim int32[n], end_trim int32[n], start scores, end scores, n_hits int32[n], hits int32[total, 10]): the
+    scores are the score pairs uint16[n, n_cols, 2] of adapter_end_decisions, or with want_top2 its int32[n, 6] ranking; the
+    hits are those of adapter_middle_scan on seq[start_trim : len - end_trim].
+    """
+    seq_buf = np.ascontiguousarray(seq_buf, dtype=np.uint8)
+    seq_off = np.ascontiguousarray(seq_off, dtype=np.int64)
+    n_seqs = len(seq_off) - 1
+    ma, mi, go, ge = [int(x) for x in scoring_scheme_vals]
+    return _trim_reads(lambda args: C_LIB.adapterTrimReads(_ptr(seq_buf), _ptr(seq_off), n_seqs, args, ma, mi, go, ge), n_seqs,
+                       start, end, middle, end_size, extra_trim_size, end_threshold, min_trim_size, middle_threshold, want_top2)
+
+
+def adapter_trim_reads_device(d_seqs_ptr, d_seq_off_ptr, n_seqs, total_seq_bytes, max_seq_len, start, end, middle,
+                              scoring_scheme_vals, end_size, extra_trim_size, end_threshold, min_trim_size, middle_threshold=85.0,
+                              want_top2=False, stream_ptr=0):
+    """adapter_trim_reads with the reads already in device memory (raw device pointers as ints, the conventions of
+    adapter_middle_scan_device).  The caller's device buffers are not modified."""
+    ma, mi, go, ge = [int(x) for x in scoring_scheme_vals]
+    return _trim_reads(lambda args: C_LIB.adapterTrimReadsDevice(
+        c_void_p(d_seqs_ptr), c_void_p(d_seq_off_ptr), n_seqs, total_seq_bytes, max_seq_len, args, ma, mi, go, ge,
+        c_void_p(stream_ptr)), int(n_seqs), start, end, middle, end_size, extra_trim_size, end_threshold, min_trim_size,
+        middle_threshold, want_top2)
 
 
 def middle_threshold_table(middle_threshold, length):

@@ -191,6 +191,9 @@ struct Engine {
     // middle-adapter scan (adapterMiddleScan*): the resident segment -- codes (masked in place), offsets, records, next adapter
     // per read, hit slots, two active lists, threshold table, append counter + longest appended read
     DevBuf mid_codes, mid_off, mid_rec, mid_next_ad, mid_hits, mid_active[2], mid_cmin, mid_ctr;
+    // whole-read trimming (adapterTrimReads*): the segment's ASCII reads and offsets (host API), window offsets, start / end
+    // windows, segment-wide start / end trims, the first base of every trimmed read, tile sums of the offset scans
+    DevBuf trim_reads, trim_off, trim_win_off, trim_win[2], trim_d[2], trim_first, trim_scan;
     // adapter-set search (adapterSetSearch): NSTAGE slices of search_cols u64 keys, one per stage, so that stages running at
     // once never share an accumulator; a batch owns the columns [search_col, search_col + n_adapters) of every slice
     DevBuf search_acc;
@@ -964,6 +967,36 @@ struct Packer {
     }
 };
 
+// decide_kernel over the records of `cnt` reads (the reads s0 .. s0+cnt-1 of decision batch D) on `stream`: the trims go to
+// d_trim (the stage's chunk scratch, or a segment-wide array that later kernels read) and are copied home with the score
+// pairs / top2 of the chunk into D's host outputs.
+int launch_decide(Engine &E, Stage &S, cudaStream_t stream, const pb200_end_batch_t &D, const int32_t *records, int64_t cnt,
+                  int32_t n_adapters, const int32_t *d_cmin, int32_t cmin_len, const int32_t *d_cols, int32_t *d_trim, int64_t s0) {
+    if (int rc = S.dec_pairs.ensure((size_t)cnt * std::max<int32_t>(D.n_score_cols, 1) * 4)) return rc;
+    DecideArgs a;
+    a.records = records; a.n = cnt; a.n_adapters = n_adapters;
+    a.is_start = D.is_start; a.end_size = D.end_size; a.extra_trim = D.extra_trim_size; a.min_trim = D.min_trim_size;
+    a.cmin = d_cmin; a.cmin_len = cmin_len; a.cols = d_cols; a.n_cols = D.n_score_cols;
+    a.trim = d_trim;
+    a.pairs = (D.score_pairs && D.n_score_cols > 0) ? S.dec_pairs.as<uint32_t>() : nullptr;
+    a.top2 = nullptr;
+    if (D.top2) {
+        if (int rc = S.dec_top2.ensure((size_t)cnt * 6 * 4)) return rc;
+        a.top2 = S.dec_top2.as<int32_t>();
+    }
+    const int64_t blocks = std::min<int64_t>((cnt + 3) / 4, (int64_t)E.sm_count * 16);
+    decide_kernel<<<(unsigned)blocks, 128, 0, stream>>>(a, S.misc.as<int>());
+    g_launches++;
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(D.trim + s0, d_trim, (size_t)cnt * 4, cudaMemcpyDeviceToHost, stream));
+    if (a.pairs)
+        CK(cudaMemcpyAsync(D.score_pairs + (size_t)s0 * D.n_score_cols * 2, S.dec_pairs.p,
+                           (size_t)cnt * D.n_score_cols * 4, cudaMemcpyDeviceToHost, stream));
+    if (a.top2)
+        CK(cudaMemcpyAsync(D.top2 + (size_t)s0 * 6, S.dec_top2.p, (size_t)cnt * 6 * 4, cudaMemcpyDeviceToHost, stream));
+    return 0;
+}
+
 // Chunks of every job flow through ONE ring of NSTAGE streams (H2D / kernels / D2H of consecutive chunks overlap, also
 // across job boundaries: no fill / drain bubble between the start-window and the end-window batch of an end-trim step).
 // Caller holds E.mu and has run E.init().
@@ -1055,30 +1088,9 @@ int run_cross_jobs(Engine &E, std::vector<CrossJob> &jobs, int ma, int mi, int g
                                               S.misc.as<int>())) return rc;
         }
         if (J.dec) {
-            const pb200_end_batch_t &D = *J.dec;
             if (int rc = S.dec_trim.ensure((size_t)cnt * 4)) return rc;
-            if (int rc = S.dec_pairs.ensure((size_t)cnt * std::max<int32_t>(D.n_score_cols, 1) * 4)) return rc;
-            DecideArgs a;
-            a.records = S.out.as<int32_t>(); a.n = cnt; a.n_adapters = J.n_adapters;
-            a.is_start = D.is_start; a.end_size = D.end_size; a.extra_trim = D.extra_trim_size; a.min_trim = D.min_trim_size;
-            a.cmin = J.d_cmin; a.cmin_len = J.cmin_len; a.cols = J.d_cols; a.n_cols = D.n_score_cols;
-            a.trim = S.dec_trim.as<int32_t>();
-            a.pairs = (D.score_pairs && D.n_score_cols > 0) ? S.dec_pairs.as<uint32_t>() : nullptr;
-            a.top2 = nullptr;
-            if (D.top2) {
-                if (int rc = S.dec_top2.ensure((size_t)cnt * 6 * 4)) return rc;
-                a.top2 = S.dec_top2.as<int32_t>();
-            }
-            const int64_t blocks = std::min<int64_t>((cnt + 3) / 4, (int64_t)E.sm_count * 16);
-            decide_kernel<<<(unsigned)blocks, 128, 0, stream>>>(a, S.misc.as<int>());
-            g_launches++;
-            CK(cudaGetLastError());
-            CK(cudaMemcpyAsync(D.trim + s0, S.dec_trim.p, (size_t)cnt * 4, cudaMemcpyDeviceToHost, stream));
-            if (a.pairs)
-                CK(cudaMemcpyAsync(D.score_pairs + (size_t)s0 * D.n_score_cols * 2, S.dec_pairs.p,
-                                   (size_t)cnt * D.n_score_cols * 4, cudaMemcpyDeviceToHost, stream));
-            if (a.top2)
-                CK(cudaMemcpyAsync(D.top2 + (size_t)s0 * 6, S.dec_top2.p, (size_t)cnt * 6 * 4, cudaMemcpyDeviceToHost, stream));
+            if (int rc = launch_decide(E, S, stream, *J.dec, S.out.as<int32_t>(), cnt, J.n_adapters, J.d_cmin, J.cmin_len, J.d_cols,
+                                       S.dec_trim.as<int32_t>(), s0)) return rc;
         }
         if (J.search_col >= 0) {
             unsigned long long *best = E.search_acc.as<unsigned long long>() + (size_t)(&S - E.st) * E.search_cols + J.search_col;
@@ -1585,17 +1597,21 @@ size_t device_free_bytes() {
 // The reads [a, b) of the next segment: its resident buffers take at most half of the free device memory (plus what the
 // engine already holds for them) and n * n_adapters stays below 2^31 (records are indexed with int32 out_idx).
 // h_seq_off: host offsets when the segment's codes are part of its resident buffers (host API), else nullptr.
-int64_t middle_segment_end(const Engine &E, int64_t a, int64_t n_seqs, int32_t n_adapters, const int64_t *h_seq_off) {
+// extra_per_read / byte_weight / extra_held: what a caller keeps resident next to the scan's buffers (adapterTrimReads: the
+// end windows per read, the ASCII reads next to their codes, and the buffers it already holds for them).
+int64_t middle_segment_end(const Engine &E, int64_t a, int64_t n_seqs, int32_t n_adapters, const int64_t *h_seq_off,
+                           double extra_per_read = 0, double byte_weight = 1, size_t extra_held = 0) {
     const size_t held = E.mid_codes.cap + E.mid_off.cap + E.mid_rec.cap + E.mid_next_ad.cap + E.mid_hits.cap +
-                        E.mid_active[0].cap + E.mid_active[1].cap;
+                        E.mid_active[0].cap + E.mid_active[1].cap + extra_held;
     const double budget = (double)(device_free_bytes() + held) / 2;
     // per read: offset, records, next adapter, hit slot, two active-list entries, the two-pass task and end-cell records
-    const double per_read = 8 + (double)n_adapters * (PB_REC * 4 + sizeof(Task) + 16) + 4 + PB_HIT_INTS * 4 + 8;
+    const double per_read = 8 + (double)n_adapters * (PB_REC * 4 + sizeof(Task) + 16) + 4 + PB_HIT_INTS * 4 + 8 + extra_per_read;
     const int64_t max_reads = std::max<int64_t>(1, std::min<int64_t>(0x7fffffffll / std::max<int32_t>(n_adapters, 1),
                                                                      (int64_t)(budget / per_read)));
     int64_t b = std::min(n_seqs, a + max_reads);
     if (h_seq_off)
-        while (b > a + 1 && (double)(h_seq_off[b] - h_seq_off[a]) + (double)(b - a) * per_read > budget) b = a + (b - a) / 2;
+        while (b > a + 1 && byte_weight * (double)(h_seq_off[b] - h_seq_off[a]) + (double)(b - a) * per_read > budget)
+            b = a + (b - a) / 2;
     return b;
 }
 
@@ -1832,6 +1848,260 @@ int middle_device(const uint8_t *d_seqs, const int64_t *d_seq_off, int64_t n_seq
     return middle_emit(rounds, n_seqs, n_hits, hits, hits_cap, n_total);
 }
 
+// ---- whole-read trimming (adapterTrimReads, Phase B + Phase C) ---------------------------------------------------------
+// Lengths in x[1 .. n] (x[0] = 0) -> their exclusive offsets in x[0 .. n], in place on `stream`.
+int scan_offsets(Engine &E, cudaStream_t stream, int64_t *x, int64_t n) {
+    if (n <= 0) return 0;
+    const int64_t tiles = (n + PB_SCAN_TILE - 1) / PB_SCAN_TILE;
+    if (int rc = E.trim_scan.ensure((size_t)tiles * 8)) return rc;
+    int64_t *sums = E.trim_scan.as<int64_t>();
+    scan_tiles_kernel<<<(unsigned)tiles, PB_SCAN_THREADS, 0, stream>>>(static_cast<const int64_t *>(x + 1), n, sums);
+    scan_tile_sums_kernel<<<1, PB_SCAN_THREADS, 0, stream>>>(sums, tiles);
+    scan_apply_kernel<<<(unsigned)tiles, PB_SCAN_THREADS, 0, stream>>>(x + 1, n, static_cast<const int64_t *>(sums));
+    g_launches += 3;
+    CK(cudaGetLastError());
+    return 0;
+}
+
+// One side of Phase B: preconditions (those of adapterEndDecisions plus int16 classes with a finite window bound) and the
+// threshold table's length.
+int trim_side_check(const pb200_trim_side_t &T, int64_t n_seqs, int32_t end_size, const SchemeInfo &si, int32_t *cmin_len) {
+    if (T.n_adapters < 0 || T.n_score_cols < 0) return fail(PB200_ERR_ARG, "negative count");
+    if (n_seqs > 0 && !T.trim) return fail(PB200_ERR_ARG, "NULL pointer");
+    if (T.n_score_cols > 0 && ((!T.score_pairs && !T.top2) || !T.score_cols)) return fail(PB200_ERR_ARG, "NULL pointer");
+    for (int32_t k = 0; k < T.n_score_cols; ++k)
+        if (T.score_cols[k] < 0 || T.score_cols[k] >= T.n_adapters) return fail(PB200_ERR_ARG, "score column out of range");
+    *cmin_len = 0;
+    if (T.n_adapters == 0) return 0;
+    if (!T.ad_off) return fail(PB200_ERR_ARG, "NULL pointer");
+    if (int rc = validate_args(nullptr, nullptr, 0, T.adapters, T.ad_off, T.n_adapters, nullptr, nullptr, 0, true)) return rc;
+    if (!si.bounded) return fail(PB200_ERR_ARG, "whole-read trimming needs negative gap scores (a finite window bound)");
+    int64_t m_max = 0;
+    for (int32_t a = 0; a < T.n_adapters; ++a) {
+        const int32_t m = T.ad_off[a + 1] - T.ad_off[a];
+        if (class_of(si, m) == GENERIC_CLASS) return fail(PB200_ERR_ARG, "adapter or scheme outside the int16 kernels");
+        m_max = std::max<int64_t>(m_max, m);
+    }
+    if ((int64_t)end_size + m_max + 2 > 65535) return fail(PB200_ERR_ARG, "windows too long for the device decisions");
+    if (T.top2 && ((int64_t)end_size + m_max + 2 > 4095 || T.n_score_cols >= 0xFFFF))
+        return fail(PB200_ERR_ARG, "windows too long / too many score columns for the device barcode ranking");
+    *cmin_len = (int32_t)(end_size + m_max + 2);
+    return 0;
+}
+
+// The reads [a, b) of the next segment: the middle scan's budget (middle_segment_end) with, per read, the two end windows (and
+// their codes when they are encoded), window offsets, two trims, the trimmed range's first base and -- host API -- the
+// segment's ASCII reads and offsets next to their codes.
+int64_t trim_segment_end(const Engine &E, int64_t a, int64_t n_seqs, int32_t n_mid, int64_t wl_max, const int64_t *h_seq_off) {
+    const size_t held = E.trim_reads.cap + E.trim_off.cap + E.trim_win_off.cap + E.trim_win[0].cap + E.trim_win[1].cap +
+                        E.trim_d[0].cap + E.trim_d[1].cap + E.trim_first.cap;
+    int64_t b = middle_segment_end(E, a, n_seqs, n_mid, h_seq_off, 3.0 * (double)wl_max + 40, h_seq_off ? 2.0 : 1.0, held);
+#ifdef PB_TEST_SEGMENT_READS
+    // tests of the host-simulated engine only (through sim_engine.load): small segments, so that a few reads span several
+    b = std::min<int64_t>(b, a + PB_TEST_SEGMENT_READS);
+#endif
+    return b;
+}
+
+// device: seqs / seq_off are device pointers (adapterTrimReadsDevice), else host buffers uploaded segment by segment.
+int trim_reads(const uint8_t *seqs, const int64_t *seq_off, int64_t n_seqs, bool device, int64_t total_seq_bytes,
+               int64_t max_seq_len, const pb200_trim_args_t *A, int ma, int mi, int go, int ge, void *user_stream) {
+    // ---- preconditions: nothing below touches the device before they all hold ----
+    if (!A) return fail(PB200_ERR_ARG, "NULL pointer");
+    if (n_seqs < 0 || total_seq_bytes < 0) return fail(PB200_ERR_ARG, "negative count");
+    if (A->end_size < 1) return fail(PB200_ERR_ARG, "end_size must be >= 1");
+    if (!(A->end_threshold >= 0.0)) return fail(PB200_ERR_ARG, "end_threshold must be >= 0 for the device decisions");
+    load_env_options();
+    const SchemeInfo si = scheme_info(ma, mi, go, ge);
+    const pb200_trim_side_t *side[2] = {&A->start, &A->end};
+    int32_t cmin_len[2] = {0, 0}, mid_cmin_len = 0;
+    for (int k = 0; k < 2; ++k)
+        if (int rc = trim_side_check(*side[k], n_seqs, A->end_size, si, &cmin_len[k])) return rc;
+    const int32_t n_mid = A->n_mid_adapters;
+    if (n_mid < 0) return fail(PB200_ERR_ARG, "negative count");
+    if (n_mid > 0) {
+        if (int rc = middle_check_outputs(n_seqs, n_mid, A->n_hits, A->hits, A->hits_cap, A->n_total)) return rc;
+        if (!A->mid_ad_off) return fail(PB200_ERR_ARG, "NULL pointer");
+        if (int rc = validate_args(nullptr, nullptr, 0, A->mid_adapters, A->mid_ad_off, n_mid, nullptr, nullptr, 0, true)) return rc;
+        if (int rc = middle_preconditions(A->mid_adapters, A->mid_ad_off, n_mid, ma, mi, go, ge, A->middle_threshold, &mid_cmin_len))
+            return rc;
+    }
+    if (n_seqs > 0 && !seq_off) return fail(PB200_ERR_ARG, "NULL pointer");
+    int64_t max_len = max_seq_len;
+    if (!device && n_seqs > 0) {
+        if (int rc = validate_args(seqs, seq_off, n_seqs, nullptr, nullptr, 0, nullptr, nullptr, 0, true)) return rc;
+        max_len = 0;
+        for (int64_t s = 0; s < n_seqs; ++s) {
+            const int64_t len = seq_off[s + 1] - seq_off[s];
+            if (len < 0) return fail(PB200_ERR_ARG, "sequence offsets not monotone");
+            max_len = std::max(max_len, len);
+        }
+    }
+    if (max_len > 0x7fff0000ll) return fail(PB200_ERR_ARG, "sequence longer than 2^31");
+    if (A->n_hits && n_seqs > 0) memset(A->n_hits, 0, (size_t)n_seqs * 4);
+    if (A->n_total) *A->n_total = 0;
+    for (int k = 0; k < 2; ++k) {         // a side without adapters: nothing aligns, nothing is trimmed
+        const pb200_trim_side_t &T = *side[k];
+        if (T.n_adapters > 0 || n_seqs == 0) continue;
+        memset(T.trim, 0, (size_t)n_seqs * 4);
+        if (T.top2) for (int64_t s = 0; s < n_seqs; ++s) { int32_t *o = T.top2 + s * 6; o[0] = o[3] = -1; o[1] = o[4] = 0; o[2] = o[5] = 1; }
+    }
+    if (n_seqs == 0 || (A->start.n_adapters == 0 && A->end.n_adapters == 0 && n_mid == 0)) return 0;
+
+    Engine *Ep = nullptr;
+    if (int rc = get_engine(&Ep)) return rc;
+    Engine &E = *Ep;
+    std::lock_guard<std::mutex> lk(E.mu);
+    if (int rc = E.init()) return rc;
+    Stage &S = E.st[0];
+    cudaStream_t stream = S.stream;
+    if (device) { if (int rc = library_stream(E, user_stream, &stream)) return rc; }
+    if (int rc = order_after_last(E, stream)) return rc;
+    NvtxRange submit_range("pb200:submit_trim");
+    std::vector<MiddleRound> rounds;
+    auto run = [&]() -> int {
+        if (int rc = reset_misc(S, stream)) return rc;
+        if (int rc = check_status(S, stream)) return rc;     // a deferred error of an earlier device-resident call
+        AdapterPlan P[2], PM;
+        for (int k = 0; k < 2; ++k) {
+            const pb200_trim_side_t &T = *side[k];
+            if (T.n_adapters == 0) continue;
+            if (int rc = plan_adapters(E, stream, T.adapters, T.ad_off, T.n_adapters, ma, mi, go, ge, P[k])) return rc;
+            const auto table = cached_threshold_table(A->end_threshold, cmin_len[k]);
+            if (int rc = E.dec_cmin[k].ensure((size_t)cmin_len[k] * 4)) return rc;
+            if (int rc = E.dec_cols[k].ensure((size_t)std::max<int32_t>(T.n_score_cols, 1) * 4)) return rc;
+            CK(cudaMemcpyAsync(E.dec_cmin[k].p, table->data(), (size_t)cmin_len[k] * 4, cudaMemcpyHostToDevice, stream));
+            if (T.n_score_cols > 0)
+                CK(cudaMemcpyAsync(E.dec_cols[k].p, T.score_cols, (size_t)T.n_score_cols * 4, cudaMemcpyHostToDevice, stream));
+        }
+        if (n_mid > 0) {
+            if (int rc = plan_adapters(E, stream, A->mid_adapters, A->mid_ad_off, n_mid, ma, mi, go, ge, PM)) return rc;
+            if (int rc = middle_table(E, stream, A->middle_threshold, mid_cmin_len)) return rc;   // (synchronises the stream)
+        }
+        if (max_len < 0) {
+            if (int rc = device_max_len(S, stream, seq_off, n_seqs, &max_len)) return rc;
+            if (max_len > 0x7fff0000ll) return fail(PB200_ERR_ARG, "sequence longer than 2^31");
+        }
+        const int64_t wl_max = std::min<int64_t>(A->end_size, max_len);
+        if (device && n_mid > 0) {
+            if (int rc = E.mid_codes.ensure((size_t)total_seq_bytes + 16)) return rc;
+        }
+        for (int64_t a = 0; a < n_seqs;) {
+            const int64_t b = trim_segment_end(E, a, n_seqs, n_mid, wl_max, device ? nullptr : seq_off);
+            const int64_t n = b - a;
+            // the segment's reads: ASCII at reads[off[s] .. off[s+1])
+            const uint8_t *reads = seqs;
+            const int64_t *off = seq_off + a;
+            int64_t bytes = 0;
+            if (!device) {                   // the only upload of read bytes
+                bytes = seq_off[b] - seq_off[a];
+                if (int rc = E.trim_reads.ensure((size_t)bytes + 16)) return rc;
+                if (int rc = E.trim_off.ensure((size_t)(n + 1) * 8)) return rc;
+                if (bytes) CK(cudaMemcpyAsync(E.trim_reads.p, seqs + seq_off[a], (size_t)bytes, cudaMemcpyHostToDevice, stream));
+                CK(cudaMemcpyAsync(E.trim_off.p, seq_off + a, (size_t)(n + 1) * 8, cudaMemcpyHostToDevice, stream));
+                rebase_kernel<<<(unsigned)((n + 1 + 255) / 256), 256, 0, stream>>>(E.trim_off.as<int64_t>(), n + 1, seq_off[a]);
+                g_launches++;
+                reads = E.trim_reads.as<uint8_t>();
+                off = E.trim_off.as<int64_t>();
+            }
+            const int64_t warp_blocks = std::max<int64_t>(1, std::min<int64_t>((n + 3) / 4, (int64_t)E.sm_count * 16));
+            // ---- end windows: lengths, offsets (shared by both sides), the cut ----
+            const size_t win_bytes = (size_t)n * (size_t)wl_max;
+            if (int rc = E.trim_win_off.ensure((size_t)(n + 1) * 8)) return rc;
+            if (int rc = E.trim_win[0].ensure(win_bytes + 16)) return rc;
+            if (int rc = E.trim_win[1].ensure(win_bytes + 16)) return rc;
+            int64_t *win_off = E.trim_win_off.as<int64_t>();
+            window_len_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(off, n, (int64_t)A->end_size, win_off);
+            g_launches++;
+            if (int rc = scan_offsets(E, stream, win_off, n)) return rc;
+            cut_windows_kernel<<<(unsigned)warp_blocks, 128, 0, stream>>>(reads, off, static_cast<const int64_t *>(win_off), n,
+                                                                         E.trim_win[0].as<uint8_t>(), E.trim_win[1].as<uint8_t>());
+            g_launches++;
+            CK(cudaGetLastError());
+            // ---- Phase B, side by side: DP chunks, then decide_kernel into the segment-wide trims ----
+            int64_t win_total = -1;
+            for (int k = 0; k < 2; ++k) {
+                const pb200_trim_side_t &T = *side[k];
+                if (int rc = E.trim_d[k].ensure((size_t)n * 4 + 16)) return rc;
+                if (T.n_adapters == 0) {
+                    CK(cudaMemsetAsync(E.trim_d[k].p, 0, (size_t)n * 4, stream));
+                    continue;
+                }
+                const bool ascii = single_pass_ascii(P[k], wl_max);
+                const uint8_t *w = E.trim_win[k].as<uint8_t>();
+                if (!ascii) {                // two-pass windows: encode first, as batch_device_queue does
+                    if (win_total < 0) {
+                        CK(cudaMemcpyAsync(&win_total, win_off + n, 8, cudaMemcpyDeviceToHost, stream));
+                        CK(cudaStreamSynchronize(stream));
+                    }
+                    if (int rc = S.seq_codes.ensure((size_t)win_total + 16)) return rc;
+                    if (int rc = launch_encode(stream, w, S.seq_codes.as<uint8_t>(), win_total, E.sm_count)) return rc;
+                    w = S.seq_codes.as<uint8_t>();
+                }
+                pb200_end_batch_t D;
+                memset(&D, 0, sizeof D);
+                D.is_start = k == 0 ? 1 : 0; D.end_size = A->end_size; D.extra_trim_size = A->extra_trim_size;
+                D.min_trim_size = A->min_trim_size; D.end_threshold = A->end_threshold;
+                D.score_cols = T.score_cols; D.n_score_cols = T.n_score_cols;
+                D.trim = T.trim; D.score_pairs = T.score_pairs; D.top2 = T.top2;
+                const int64_t max_cnt = std::max<int64_t>(1, g_opt.device_chunk_tasks / T.n_adapters);
+                for (int64_t c0 = 0; c0 < n; c0 += max_cnt) {
+                    const int64_t cnt = std::min(max_cnt, n - c0);
+                    if (int rc = S.out.ensure((size_t)cnt * T.n_adapters * PB_REC * 4)) return rc;
+                    if (int rc = run_cross_chunk(E, S, stream, P[k], w, win_off + c0, cnt, 0, wl_max, T.n_adapters,
+                                                 S.out.as<int32_t>(), nullptr, 0, T.ad_off, nullptr, ascii)) return rc;
+                    if (int rc = launch_decide(E, S, stream, D, S.out.as<int32_t>(), cnt, T.n_adapters, E.dec_cmin[k].as<int32_t>(),
+                                               cmin_len[k], E.dec_cols[k].as<int32_t>(), E.trim_d[k].as<int32_t>() + c0, a + c0))
+                        return rc;
+                }
+            }
+            if (n_mid == 0) {
+                if (int rc = check_status(S, stream)) return rc;
+                a = b;
+                continue;
+            }
+            // ---- trims -> trimmed reads, encoded into the middle scan's resident codes ----
+            MiddleSeg M;
+            if (int rc = middle_segment_buffers(E, n, n_mid, device ? 0 : (size_t)bytes, M)) return rc;
+            if (int rc = E.trim_first.ensure((size_t)n * 8 + 16)) return rc;
+            M.codes = E.mid_codes.as<uint8_t>();
+            M.off = E.mid_off.as<int64_t>();
+            M.cmin_len = mid_cmin_len;
+            trimmed_range_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(off, static_cast<const int32_t *>(E.trim_d[0].as<int32_t>()),
+                                                                                 static_cast<const int32_t *>(E.trim_d[1].as<int32_t>()), n,
+                                                                                 E.trim_first.as<int64_t>(), M.off);
+            g_launches++;
+            if (int rc = scan_offsets(E, stream, M.off, n)) return rc;
+            gather_encode_kernel<<<(unsigned)warp_blocks, 128, 0, stream>>>(reads, off, static_cast<const int64_t *>(E.trim_first.as<int64_t>()),
+                                                                           static_cast<const int64_t *>(M.off), n, M.codes);
+            g_launches++;
+            CK(cudaGetLastError());
+            if (int rc = device_max_len(S, stream, M.off, n, &M.max_len)) return rc;
+            // ---- Phase C: round 0 over every trimmed read, then the masking rounds, as in middle_device ----
+            CK(cudaMemsetAsync(E.mid_ctr.p, 0, 16, stream));
+            const int64_t max_cnt = std::max<int64_t>(1, g_opt.device_chunk_tasks / n_mid);
+            for (int64_t c0 = 0; c0 < n; c0 += max_cnt) {
+                const int64_t cnt = std::min(max_cnt, n - c0);
+                if (int rc = run_cross_chunk(E, S, stream, PM, M.codes, M.off + c0, cnt, 0, M.max_len, n_mid,
+                                             M.rec + (size_t)c0 * n_mid * PB_REC, nullptr, 0, A->mid_ad_off)) return rc;
+                if (int rc = launch_middle_decide(E, stream, M, n_mid, nullptr, c0, cnt, M.active[0], S.misc.as<int>())) return rc;
+            }
+            if (int rc = middle_rounds(E, S, stream, PM, M, n_mid, A->mid_ad_off, a, rounds)) return rc;
+            a = b;
+        }
+        return 0;
+    };
+    const int rc = run();
+    if (rc) {                             // nothing may still be running (or writing the caller's outputs) when we return
+        const std::string first_err = g_err;
+        cudaStreamSynchronize(stream);
+        g_err = first_err;
+    }
+    E.last_pending = false;               // the stream waited for an earlier call's queued work, and all of it is done
+    if (rc || n_mid == 0) return rc;
+    return middle_emit(rounds, n_seqs, A->n_hits, A->hits, A->hits_cap, A->n_total);
+}
+
 }  // namespace
 
 // =====================================================================================================
@@ -1880,6 +2150,18 @@ int adapterMiddleScanDevice(const uint8_t *d_seqs, const int64_t *d_seq_off, int
     g_err.clear();
     return middle_device(d_seqs, d_seq_off, n_seqs, total_seq_bytes, max_seq_len, adapters, ad_off, n_adapters, ma, mi, go, ge,
                          middle_threshold, n_hits, hits, hits_cap, n_total, stream);
+}
+
+int adapterTrimReads(const uint8_t *seqs, const int64_t *seq_off, int64_t n_seqs, const pb200_trim_args_t *args, int ma, int mi,
+                     int go, int ge) {
+    g_err.clear();
+    return trim_reads(seqs, seq_off, n_seqs, false, 0, -1, args, ma, mi, go, ge, nullptr);
+}
+
+int adapterTrimReadsDevice(const uint8_t *d_seqs, const int64_t *d_seq_off, int64_t n_seqs, int64_t total_seq_bytes,
+                           int64_t max_seq_len, const pb200_trim_args_t *args, int ma, int mi, int go, int ge, void *stream) {
+    g_err.clear();
+    return trim_reads(d_seqs, d_seq_off, n_seqs, true, total_seq_bytes, max_seq_len, args, ma, mi, go, ge, stream);
 }
 
 int pb200MiddleThresholdTable(double middle_threshold, int32_t len, int32_t *cmin) {

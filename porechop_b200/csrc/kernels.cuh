@@ -9,6 +9,8 @@
 //   decide_kernel        records -> per-read end-trim amounts + barcode score pairs (decisions stay on the device)
 //   search_best_kernel   records -> per-adapter best full-adapter identity of the adapter-set search (Phase A)
 //   middle_decide_kernel one round of the middle-adapter scan: first hit per active read, masking, next active list
+//   window_len / cut_windows / trimmed_range / gather_encode + scan_*: whole-read trimming (adapterTrimReads) -- end windows
+//                        cut from resident reads, trims turned into the trimmed reads the middle scan masks
 //   generic_kernel       int32 thread-serial fallback for scoring schemes / adapters outside the int16 domain
 //
 // The arithmetic is in dp_core.cuh (shared with the CPU emulation used by the tests).
@@ -946,6 +948,132 @@ __global__ void middle_decide_kernel(const MiddleArgs a, int *__restrict__ statu
         if (lane < PB_HIT_INTS) a.hits[(size_t)pos * PB_HIT_INTS + lane] = lane == 0 ? hit : r[lane - 1];
     }
     if (ovf) atomicOr(status, 2);
+}
+
+// ---------------------------------------------------------------------------------------------------
+// Whole-read trimming (adapterTrimReads): the glue between resident reads, the end-window DP of Phase B and the middle scan.
+// Reads are ASCII at reads[off[s] .. off[s+1]); every kernel takes plain pointers (const = read, non-const = written).
+//
+// Lengths -> offsets: a length kernel writes len[s] into x[s+1] (and 0 into x[0]); the three scan kernels then turn
+// x[1 .. n] into its inclusive prefix sums in place (reduce per tile, scan the tile sums in one block, scan each tile with its
+// prefix), so that x becomes the exclusive offsets of the lengths.  A tile is PB_SCAN_THREADS x PB_SCAN_ITEMS values.
+constexpr int PB_SCAN_THREADS = 256;
+constexpr int PB_SCAN_ITEMS = 8;
+constexpr int64_t PB_SCAN_TILE = (int64_t)PB_SCAN_THREADS * PB_SCAN_ITEMS;
+
+// exclusive scan of one value per thread over the block (blockDim.x a multiple of 32); *total = the block's sum
+__device__ __forceinline__ long long block_exclusive_scan(long long v, long long *total) {
+    __shared__ long long warp_tot[32];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, n_warps = blockDim.x >> 5;
+    long long inc = v;
+    for (int o = 1; o < 32; o <<= 1) {
+        const long long t = __shfl_up_sync(0xffffffffu, inc, o);
+        if (lane >= o) inc += t;
+    }
+    if (lane == 31) warp_tot[warp] = inc;
+    __syncthreads();
+    if (warp == 0) {
+        long long w = lane < n_warps ? warp_tot[lane] : 0;
+        for (int o = 1; o < 32; o <<= 1) {
+            const long long t = __shfl_up_sync(0xffffffffu, w, o);
+            if (lane >= o) w += t;
+        }
+        if (lane < n_warps) warp_tot[lane] = w;          // inclusive over the warps
+    }
+    __syncthreads();
+    const long long excl = inc - v + (warp ? warp_tot[warp - 1] : 0);
+    *total = warp_tot[n_warps - 1];
+    __syncthreads();                                       // warp_tot may be reused by the caller's next scan
+    return excl;
+}
+// tile sums of x[0 .. n): one block per tile
+__global__ void scan_tiles_kernel(const int64_t *x, int64_t n, int64_t *tile_sums) {
+    const int64_t base = (int64_t)blockIdx.x * PB_SCAN_TILE + (int64_t)threadIdx.x * PB_SCAN_ITEMS;
+    long long s = 0;
+    for (int k = 0; k < PB_SCAN_ITEMS; ++k) if (base + k < n) s += x[base + k];
+    long long total = 0;
+    block_exclusive_scan(s, &total);
+    if (threadIdx.x == 0) tile_sums[blockIdx.x] = total;
+}
+// exclusive scan of the n tile sums in place: one block, each thread a contiguous run
+__global__ void scan_tile_sums_kernel(int64_t *tile_sums, int64_t n) {
+    const int64_t per = (n + blockDim.x - 1) / blockDim.x;
+    const int64_t lo = (int64_t)threadIdx.x * per, hi = lo + per < n ? lo + per : n;
+    long long s = 0;
+    for (int64_t i = lo; i < hi; ++i) s += tile_sums[i];
+    long long total = 0;
+    long long run = block_exclusive_scan(s, &total);
+    for (int64_t i = lo; i < hi; ++i) { const long long v = tile_sums[i]; tile_sums[i] = run; run += v; }
+}
+// inclusive scan of x[0 .. n) in place, tile by tile from the tile's exclusive prefix
+__global__ void scan_apply_kernel(int64_t *x, int64_t n, const int64_t *tile_sums) {
+    const int64_t base = (int64_t)blockIdx.x * PB_SCAN_TILE + (int64_t)threadIdx.x * PB_SCAN_ITEMS;
+    long long v[PB_SCAN_ITEMS], s = 0;
+#pragma unroll
+    for (int k = 0; k < PB_SCAN_ITEMS; ++k) { v[k] = base + k < n ? x[base + k] : 0; s += v[k]; }
+    long long total = 0;
+    long long run = block_exclusive_scan(s, &total) + tile_sums[blockIdx.x];
+#pragma unroll
+    for (int k = 0; k < PB_SCAN_ITEMS; ++k) {
+        run += v[k];
+        if (base + k < n) x[base + k] = run;
+    }
+}
+
+// window lengths min(len, end_size) of every read -> wl[s + 1] (wl[0] = 0): scanned, the offsets of the start windows and of the
+// end windows alike
+__global__ void window_len_kernel(const int64_t *off, int64_t n, int64_t end_size, int64_t *wl) {
+    const int64_t s = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (s == 0) wl[0] = 0;
+    if (s < n) {
+        const int64_t len = off[s + 1] - off[s];
+        wl[s + 1] = len < end_size ? len : end_size;
+    }
+}
+// seq[:wl] and seq[len - wl:] of every read (ASCII, nanopore_read.py:172,194) -> the two window batches; one warp per read
+__global__ void cut_windows_kernel(const uint8_t *reads, const int64_t *off, const int64_t *win_off, int64_t n, uint8_t *start,
+                                   uint8_t *end) {
+    const int lane = threadIdx.x & 31;
+    const int64_t warps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    for (int64_t s = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; s < n; s += warps) {
+        const int64_t w0 = win_off[s], wl = win_off[s + 1] - w0, tail = off[s + 1] - wl;
+        for (int64_t k = lane; k < wl; k += 32) {
+            start[w0 + k] = reads[off[s] + k];
+            end[w0 + k] = reads[tail + k];
+        }
+    }
+}
+// [a, b) of seq[start_trim : len - end_trim] with Python's slice semantics (fastq.trimmed_ranges, nanopore_read.py:57-63): an
+// end position below 0 counts from the end of the read again, an untouched read keeps [0, len).  first[s] = a,
+// lens[s + 1] = b - a (lens[0] = 0) for the scan into the trimmed reads' offsets.
+__global__ void trimmed_range_kernel(const int64_t *off, const int32_t *start_trim, const int32_t *end_trim, int64_t n,
+                                     int64_t *first, int64_t *lens) {
+    const int64_t s = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (s == 0) lens[0] = 0;
+    if (s >= n) return;
+    const int64_t len = off[s + 1] - off[s], st = start_trim[s], et = end_trim[s];
+    int64_t a = 0, b = len;
+    if (st != 0 || et != 0) {
+        int64_t e = len - et;
+        if (e < 0) e = e + len > 0 ? e + len : 0;
+        a = st < len ? st : len;
+        b = e < len ? e : len;
+        if (b < a) b = a;
+    }
+    first[s] = a;
+    lens[s + 1] = b - a;
+}
+// the trimmed reads, encoded on the way (the bytes encode_kernel writes), into the middle scan's resident codes at dst_off;
+// one warp per read
+__global__ void gather_encode_kernel(const uint8_t *reads, const int64_t *off, const int64_t *first, const int64_t *dst_off,
+                                     int64_t n, uint8_t *codes) {
+    const int lane = threadIdx.x & 31;
+    const int64_t warps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    for (int64_t s = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; s < n; s += warps) {
+        const uint8_t *src = reads + off[s] + first[s];
+        const int64_t d0 = dst_off[s], len = dst_off[s + 1] - d0;
+        for (int64_t k = lane; k < len; k += 32) codes[d0 + k] = (uint8_t)encode_byte(src[k]);
+    }
 }
 
 // ---------------------------------------------------------------------------------------------------

@@ -377,11 +377,7 @@ def find_middle_hits(batch, start_trim, end_trim, adapters, middle_threshold, sc
             if e.code != W.ERR_ARG:
                 raise
         else:
-            full, _, rs, re_ = scores_from_records(np.ascontiguousarray(h[:, 1:]))
-            reads = np.repeat(np.arange(n), n_hits)
-            for k in range(len(h)):
-                hits.setdefault(int(reads[k]), []).append((int(h[k, 0]), int(rs[k]), int(re_[k]), float(full[k])))
-            return hits
+            return _hits_dict(n_hits, h)
     rec = W.adapter_alignment_batch(tbuf, toff, abuf, aoff, scoring_scheme_vals)
     full, _, rs, re_ = (x.reshape(n, n_ad) for x in scores_from_records(rec))
     hit = full >= middle_threshold                           # NaN never hits, as in the reference
@@ -412,6 +408,16 @@ def find_middle_hits(batch, start_trim, end_trim, adapters, middle_threshold, sc
                 still.append([i, masked, p + int(h[0])])
             base += cnt
         active = still
+    return hits
+
+
+def _hits_dict(n_hits, h):
+    """n_hits / hits of adapterMiddleScan (or adapterTrimReads) -> the dict find_middle_hits returns"""
+    hits = {}
+    full, _, rs, re_ = scores_from_records(np.ascontiguousarray(h[:, 1:]))
+    reads = np.repeat(np.arange(len(n_hits)), n_hits)
+    for k in range(len(h)):
+        hits.setdefault(int(reads[k]), []).append((int(h[k, 0]), int(rs[k]), int(re_[k]), float(full[k])))
     return hits
 
 
@@ -618,21 +624,65 @@ def _middle_adapters(sets):
     return adapters
 
 
+def _trim_reads_fused(batch, starts, ends, adapters, scoring_scheme_vals, end_size, extra_end_trim, end_threshold,
+                      min_trim_size, middle_threshold, score_cols, rank_names):
+    """Phase B + Phase C in one adapterTrimReads call: the reads go up once, and the trims, the score outputs and the hits come
+    back.  Returns what trim_end_adapters (device decisions) and find_middle_hits (device scan) return together, or None when
+    the engine does not take these inputs (PB200_ERR_ARG): the caller then runs the two calls."""
+    scols, ecols = score_cols if score_cols is not None else ((), ())
+    sa, so = W.pack_sequences(starts, offset_dtype=np.int32)
+    ea, eo = W.pack_sequences(ends, offset_dtype=np.int32)
+    middle = W.pack_sequences([x[1] for x in adapters], offset_dtype=np.int32) if adapters else None
+    seq = batch.seq
+    pinned = getattr(W, 'pinned_buffer', None)
+    if pinned is not None and hostio.LIB is not None and len(seq):
+        # the bases go up from the engine's pinned staging buffer (DMA at PCIe speed): the upload of a pageable batch is staged
+        # by the driver and took longer than this parallel copy (64 KB pieces for the copy's thread team) plus the DMA
+        piece = 1 << 16
+        a = np.arange(0, len(seq), piece, dtype=np.int64)
+        seq, _ = hostio.gather(seq, a, np.minimum(piece, len(seq) - a), alloc=lambda nbytes: pinned(0, nbytes))
+    try:
+        st, et, sp, ep, n_hits, h = W.adapter_trim_reads(
+            seq, batch.seq_off, (sa, so, list(scols)), (ea, eo, list(ecols)), middle, scoring_scheme_vals, end_size,
+            extra_end_trim, end_threshold, min_trim_size, middle_threshold, want_top2=rank_names is not None)
+    except W.EngineError as e:
+        if e.code != W.ERR_ARG:
+            raise
+        return None
+    if rank_names is not None:
+        srec, erec = Top2Scores(rank_names[0], sp), Top2Scores(rank_names[1], ep)
+    else:
+        srec, erec = PairScores(scols, sp), PairScores(ecols, ep)
+    return st.astype(np.int64), et.astype(np.int64), srec, erec, _hits_dict(n_hits, h)
+
+
 def _run_trim(data, matching_sets, scoring_scheme_vals, end_size, extra_end_trim, end_threshold, min_trim_size, no_split,
-              middle_threshold, good_side, bad_side, score_cols=None, rank_names=None):
+              middle_threshold, good_side, bad_side, score_cols=None, rank_names=None, device_trim=None):
+    """device_trim (default: both DEVICE_DECISIONS and DEVICE_MIDDLE): Phase B and Phase C in one adapterTrimReads call
+    instead of adapterEndDecisions + adapterMiddleScan; inputs that call does not take run the two calls."""
     t0 = time.perf_counter()
     batch = data if isinstance(data, FastqBatch) else parse_fastq(data)
     t1 = time.perf_counter()
     sets = _norm_sets(matching_sets)
     starts = [s[1] for _, s, _ in sets if s]
     ends = [e[1] for _, _, e in sets if e]
-    st, et, srec, erec = trim_end_adapters(batch, starts, ends, scoring_scheme_vals, end_size, extra_end_trim,
-                                           end_threshold, min_trim_size, score_cols=score_cols, rank_names=rank_names)
-    t2 = time.perf_counter()
+    adapters = [] if no_split else _middle_adapters(sets)
+    if device_trim is None:
+        device_trim = DEVICE_DECISIONS and DEVICE_MIDDLE
+    fused = None
+    if device_trim and len(batch) > 0 and end_threshold >= 0 and (starts or ends):
+        fused = _trim_reads_fused(batch, starts, ends, adapters, scoring_scheme_vals, end_size, extra_end_trim, end_threshold,
+                                  min_trim_size, middle_threshold, score_cols, rank_names)
+    if fused is not None:
+        st, et, srec, erec, hits = fused
+        t2 = time.perf_counter()
+    else:
+        st, et, srec, erec = trim_end_adapters(batch, starts, ends, scoring_scheme_vals, end_size, extra_end_trim,
+                                               end_threshold, min_trim_size, score_cols=score_cols, rank_names=rank_names)
+        t2 = time.perf_counter()
+        hits = {} if no_split else find_middle_hits(batch, st, et, adapters, middle_threshold, scoring_scheme_vals)
     middle = {}
     if not no_split:
-        adapters = _middle_adapters(sets)
-        hits = find_middle_hits(batch, st, et, adapters, middle_threshold, scoring_scheme_vals)
         middle = middle_trim_ranges(hits, adapters, {s[0] for _, s, _ in sets if s}, {e[0] for _, _, e in sets if e},
                                     good_side, bad_side)
     seconds = {'parse': t1 - t0, 'end_trim': t2 - t1, 'middle': time.perf_counter() - t2}
@@ -641,14 +691,17 @@ def _run_trim(data, matching_sets, scoring_scheme_vals, end_size, extra_end_trim
 
 def trim_fastq(data, matching_sets, scoring_scheme_vals, end_size=150, extra_end_trim=2, end_threshold=75.0,
                min_trim_size=4, no_split=False, middle_threshold=85.0, extra_middle_trim_good_side=10,
-               extra_middle_trim_bad_side=100, min_split_read_size=1000, discard_middle=False, fmt='fastq', as_array=False):
+               extra_middle_trim_bad_side=100, min_split_read_size=1000, discard_middle=False, fmt='fastq', as_array=False,
+               device_trim=None):
     """FASTQ bytes -> the bytes `porechop -i in.fastq -o out.<fmt>` writes once Phase A has chosen `matching_sets`
     (porechop.py:54-79).  matching_sets: list of (start, end) with start / end = (name, sequence) or None -- the
     `start_sequence` / `end_sequence` of the reference's Adapter objects (adapters.py:18-30).
+    device_trim: see _run_trim (default: one adapterTrimReads call when DEVICE_DECISIONS and DEVICE_MIDDLE are both on).
     Returns (output bytes, info dict with the per-read decisions)."""
     batch, _, st, et, _, _, middle, seconds = _run_trim(data, matching_sets, scoring_scheme_vals, end_size, extra_end_trim,
                                                         end_threshold, min_trim_size, no_split, middle_threshold,
-                                                        extra_middle_trim_good_side, extra_middle_trim_bad_side)
+                                                        extra_middle_trim_good_side, extra_middle_trim_bad_side,
+                                                        device_trim=device_trim)
     t0 = time.perf_counter()
     out = emit(batch, st, et, middle, fmt, min_split_read_size, discard_middle, as_array=as_array)
     seconds['emit'] = time.perf_counter() - t0

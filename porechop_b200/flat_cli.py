@@ -16,7 +16,9 @@ Opt-in device paths (environment, off by default; output bytes are the same): PB
 decisions on the device (adapterEndDecisions), PB200_DEVICE_MIDDLE=1 runs the whole middle-adapter scan there, masking
 rounds included (adapterMiddleScan; inputs it does not take -- e.g. adapters with other bases than A/C/G/T/U -- use the
 host rounds), PB200_CHECK_ALL_READS=1 runs Phase A over every read, and PB200_DEVICE_SEARCH=1 reduces Phase A's records to
-one best score per adapter sequence on the device (adapterSetSearch) -- what makes checking every read cheap.
+one best score per adapter sequence on the device (adapterSetSearch) -- what makes checking every read cheap.  With
+PB200_DEVICE_DECISIONS=1 and PB200_DEVICE_MIDDLE=1 both set, each chunk's Phase B and Phase C are one engine call
+(adapterTrimReads): the reads are uploaded once and the windows, trims and trimmed reads are made on the device.
 
 Multi-GPU: launched with torchrun (one process per GPU) chunk c is handled by rank c % world on its own device; ranks
 write self-contained pieces and rank 0 stitches them in chunk order after a barrier -- no data-path collective

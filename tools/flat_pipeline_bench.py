@@ -6,6 +6,7 @@ metric (bench.py measures the alignment path itself); this is the tool for findi
     python tools/flat_pipeline_bench.py --reads 200000 --repeat 3
     python tools/flat_pipeline_bench.py --reads 200000 --middle both    # Phase C: host rounds vs adapterMiddleScan
     python tools/flat_pipeline_bench.py --reads 200000 --search both    # Phase A over every read: host vs adapterSetSearch
+    python tools/flat_pipeline_bench.py --reads 200000 --trim both      # Phase B + C: two device calls vs adapterTrimReads
 
 --middle host|device|both times Phase C with the host masking rounds (fastq.find_middle_hits' default) and / or the device
 scan (PB200_DEVICE_MIDDLE), alternating the two over the same FASTQ; it reports per path the `middle` seconds of trim_fastq,
@@ -17,6 +18,13 @@ sets, what PB200_CHECK_ALL_READS=1 does) with the record path (fastq.search_adap
 reduction (PB200_DEVICE_SEARCH), alternating the two over the same FASTQ; it reports per path the seconds of
 search_adapter_sets and the bytes it copies in each direction (counted from the shapes of the engine calls), the card and its
 power limit, and asserts that both paths return identical scores.
+
+--trim separate|fused|both times Phase B + Phase C with both device switches on (PB200_DEVICE_DECISIONS and
+PB200_DEVICE_MIDDLE): adapterEndDecisions over host-cut windows + adapterMiddleScan over host-gathered trimmed reads
+('separate') and / or one adapterTrimReads call ('fused'), alternating the two over the same FASTQ; it reports per path the
+`end_trim + middle` seconds of trim_fastq (best run and every run), the engine calls and the bytes they copy in each
+direction (counted from the shapes of the calls), the card and its power limit, and asserts that both paths write identical
+bytes.
 """
 import argparse
 import json
@@ -145,6 +153,83 @@ def run_middle(n_reads, repeat, which, seed=20260923):
             'paths': res}
 
 
+def _trim_counter(W):
+    """wraps the engine calls of Phase B + Phase C with both device switches on: calls and bytes each way, from the shapes of
+    what crosses the C-ABI (per masking round: hit count, longest read and status word come back)"""
+    st = {'calls': 0, 'h2d_bytes': 0, 'd2h_bytes': 0}
+    orig = (W.adapter_end_decisions, W.adapter_middle_scan, W.adapter_trim_reads)
+
+    def hit_bytes(n_hits, hits):
+        rounds = int(n_hits.max()) + 1 if len(n_hits) else 0
+        return rounds * 16 + len(hits) * (4 + hits.shape[1] * 4)
+
+    def dec(batches, scoring, *a, **k):
+        outs = orig[0](batches, scoring, *a, **k)
+        st['calls'] += 1
+        for b, (trim, scores, _) in zip(batches, outs):
+            st['h2d_bytes'] += sum(x.nbytes for x in b[:4]) + 4 * len(b[5] or ())
+            st['d2h_bytes'] += trim.nbytes + scores.nbytes
+        return outs
+
+    def scan(seq_buf, seq_off, ad_buf, ad_off, scoring, thr):
+        n_hits, hits = orig[1](seq_buf, seq_off, ad_buf, ad_off, scoring, thr)
+        st['calls'] += 1
+        st['h2d_bytes'] += seq_buf.nbytes + seq_off.nbytes + ad_buf.nbytes + ad_off.nbytes
+        st['d2h_bytes'] += hit_bytes(n_hits, hits)
+        return n_hits, hits
+
+    def trim(seq_buf, seq_off, start, end, middle, *a, **k):
+        r = orig[2](seq_buf, seq_off, start, end, middle, *a, **k)
+        st['calls'] += 1
+        st['h2d_bytes'] += seq_buf.nbytes + seq_off.nbytes + sum(x[0].nbytes + x[1].nbytes + 4 * len(x[2]) for x in (start, end)) + \
+            (middle[0].nbytes + middle[1].nbytes if middle is not None else 0)
+        st['d2h_bytes'] += r[0].nbytes + r[1].nbytes + r[2].nbytes + r[3].nbytes + hit_bytes(r[4], r[5])
+        return r
+    return st, (dec, scan, trim), orig
+
+
+def run_trim(n_reads, repeat, which, seed=20260923):
+    """Phase B + Phase C with both device switches on: adapterEndDecisions + adapterMiddleScan ('separate') against one
+    adapterTrimReads call ('fused'), alternated over the same FASTQ"""
+    import hashlib
+    from porechop_b200 import fastq, workloads as wl
+    data, (yt, yb), _ = synthetic_fastq(n_reads, seed)
+    sets = [(('SQK-NSK007_Y_Top', yt), ('SQK-NSK007_Y_Bottom', yb))]
+    paths = ['separate', 'fused'] if which == 'both' else [which]
+    res, digests = {p: None for p in paths}, {}
+    W = fastq.W
+    fastq.DEVICE_DECISIONS = fastq.DEVICE_MIDDLE = True
+    try:
+        warm, _, _ = synthetic_fastq(max(n_reads // 50, 1), seed + 1)
+        for p in paths:                                       # warm-up: plans, buffers, modules
+            fastq.trim_fastq(warm, sets, wl.DEFAULT_SCORING, as_array=True, device_trim=p == 'fused')
+        for _ in range(repeat):
+            for p in paths:                                   # alternated: the host's other work hits both alike
+                st, (dec, scan, trim), orig = _trim_counter(W)
+                W.adapter_end_decisions, W.adapter_middle_scan, W.adapter_trim_reads = dec, scan, trim
+                try:
+                    out, info = fastq.trim_fastq(data, sets, wl.DEFAULT_SCORING, as_array=True, device_trim=p == 'fused')
+                finally:
+                    W.adapter_end_decisions, W.adapter_middle_scan, W.adapter_trim_reads = orig
+                digests.setdefault(p, hashlib.sha256(out).hexdigest())
+                assert digests[p] == hashlib.sha256(out).hexdigest()
+                s = info['seconds']
+                cur = {'end_trim_middle_s': s['end_trim'] + s['middle'], 'end_trim_s': s['end_trim'], 'middle_s': s['middle'],
+                       'engine_calls': st['calls'], 'h2d_bytes': st['h2d_bytes'], 'd2h_bytes': st['d2h_bytes'],
+                       'split_reads': len(info['middle'])}
+                if res[p] is None:
+                    res[p] = dict(cur, runs_end_trim_middle_s=[])
+                res[p]['runs_end_trim_middle_s'].append(cur['end_trim_middle_s'])
+                if cur['end_trim_middle_s'] <= min(res[p]['runs_end_trim_middle_s']):
+                    res[p].update(cur)
+    finally:
+        fastq.DEVICE_DECISIONS = fastq.DEVICE_MIDDLE = False
+    if len(paths) == 2:
+        assert digests['separate'] == digests['fused'], 'the separate and the fused calls wrote different output'
+    return {'reads': n_reads, 'in_bytes': len(data), 'card': card(), 'repeat': repeat,
+            'identical_output': len(set(digests.values())) == 1, 'paths': res}
+
+
 def _phase_a_counter(W):
     """wraps the engine calls of search_adapter_sets: bytes each way, from the shapes of what crosses the C-ABI"""
     st = {'h2d_bytes': 0, 'd2h_bytes': 0}
@@ -208,8 +293,12 @@ if __name__ == '__main__':
                     help='time Phase C with the host rounds, the device scan, or both alternately')
     ap.add_argument('--search', choices=['host', 'device', 'both'], default=None,
                     help='time Phase A over every read with the record path, the device reduction, or both alternately')
+    ap.add_argument('--trim', choices=['separate', 'fused', 'both'], default=None,
+                    help='time Phase B + C with the two device calls, the one fused call, or both alternately')
     a = ap.parse_args()
-    if a.search:
+    if a.trim:
+        print(json.dumps(run_trim(a.reads, a.repeat, a.trim)))
+    elif a.search:
         print(json.dumps(run_search(a.reads, a.repeat, a.search)))
     elif a.middle:
         print(json.dumps(run_middle(a.reads, a.repeat, a.middle)))

@@ -84,5 +84,28 @@ for opts in ({}, {'direct_max': 100, 'chunk_tasks': 200}):
             exp.append(np.maximum(full.max(axis=0), 0.0))
         return np.concatenate(got), np.concatenate(exp)
     run('search', opts, search)
+# whole-read trimming (adapterTrimReads / adapterTrimReadsDevice): against adapterEndDecisions over host-cut windows +
+# adapterMiddleScan over the host-gathered trimmed reads, with one-pass (150) and two-pass (200) windows
+from porechop_b200 import fastq                     # noqa: E402
+sides = (wl.pack_adapters([yt]) + ([0],), wl.pack_adapters([yb]) + ([0],))
+for end_size in (150, 200):
+    def trim(device=False):
+        if device:
+            import torch
+            d_buf, d_off = torch.from_numpy(lbuf).cuda(), torch.from_numpy(loff).cuda()
+            got = W.adapter_trim_reads_device(d_buf.data_ptr(), d_off.data_ptr(), len(loff) - 1, len(lbuf), -1, sides[0], sides[1],
+                                              (a2, o2), wl.DEFAULT_SCORING, end_size, 2, 75.0, 4, 85.0)
+        else:
+            got = W.adapter_trim_reads(lbuf, loff, sides[0], sides[1], (a2, o2), wl.DEFAULT_SCORING, end_size, 2, 75.0, 4, 85.0)
+        (sw, swo), (ew, ewo) = fastq.end_windows(lbuf, loff, end_size)
+        (st, sp, _), (et, ep, _) = W.adapter_end_decisions([(sw, swo) + sides[0][:2] + (True, [0]), (ew, ewo) + sides[1][:2] + (False, [0])],
+                                                           wl.DEFAULT_SCORING, end_size, 2, 75.0, 4)
+        a, b = fastq.trimmed_ranges(np.diff(loff), st, et)
+        tb, to = fastq._gather_ranges(lbuf, loff[:-1] + a, loff[:-1] + b)
+        n_hits, h = W.adapter_middle_scan(tb, to, a2, o2, wl.DEFAULT_SCORING, 85.0)
+        flat = lambda xs: np.concatenate([np.asarray(x, dtype=np.int64).ravel() for x in xs])    # noqa: E731
+        return flat(got), flat((st, et, sp, ep, n_hits, h))
+    run('trim', {}, trim)
+    run('trim_dev', {}, lambda: trim(True))
 print('SANITIZE RUN COMPLETE, %d wrong' % bad, flush=True)
 sys.exit(1 if bad else 0)
