@@ -34,7 +34,8 @@ constexpr int PB_WARPS_PER_BLOCK = 4;
 #ifndef PB_TRACE_MIN_BLOCKS_WIDE
 #define PB_TRACE_MIN_BLOCKS_WIDE 5
 #endif
-constexpr int PB_SCRATCH_WORDS = 32 * 2 * 6;   // ScoutCand per lane per half
+constexpr int PB_TB_WORDS = 16 * 12;           // TbTask per half of the (at most 8) slots of a warp
+constexpr int PB_SCRATCH_WORDS = 32 * 2 * 6 + PB_TB_WORDS;   // ScoutCand per lane per half, then the TbTasks
 constexpr int PB_TCHUNK = 4;                   // trace steps per 128-bit store (must stay 4: uint4)
 
 // ---------------------------------------------------------------------------------------------------
@@ -279,6 +280,73 @@ __device__ __forceinline__ void stage_columns(uint32_t *hbuf, int g, const uint8
     }
 }
 
+// What the traceback of one half needs from its Task: written to shared memory at slot set-up by the lane that later traces
+// the half, so the traceback does not synthesise the Task a second time.  (Keeping n and m here rather than taking them from
+// the forward pass's registers also keeps the end-trim classes free of spills.)
+struct TbTask {
+    int32_t out_idx, flags, col0, n_total, ad_off, end_j, end_i, end_score, n, m, pad0, pad1;   // flags: TASK_* | end_corr << 8
+};
+static_assert(sizeof(TbTask) * 16 == PB_TB_WORDS * 4, "PB_TB_WORDS holds 16 TbTasks");
+
+// Cursor of trace_kernel's traceback over the trace of one half (see traceback_stats_cur).  The current cell (column j,
+// group row q = i + pad - 1) is lane gg = q / R, row r = q % R, step t = j - 1 + gg; its flags are the nibble of row r in
+// the trace word of step t, which is word t & 3 of the 128-bit chunk (lane gg, steps t & ~3).  Everything moves
+// incrementally: `k` indexes the chunk, `u` = t & 3, and `s` shifts row r's nibble to the top of the word (a move up one
+// row adds 4; from row 0 it wraps to row R-1 of lane gg - 1, which is also one step earlier).  A move loads nothing: the
+// chunk is fetched by the next flags(), which the caller only asks for inside the matrix.
+template <int R, int WPS>
+struct TraceCursor {
+    const uint4 *base;         // chunk 0 of lane 0 of the group (this half's words)
+    const uint32_t *hp;        // staged column word of the current column
+    const uint8_t *ap;         // adapter code of the current row
+    uint4 cv;                  // base[k] once loaded
+    int k;                     // chunk of the current cell: (t >> 2) * WPS * 32 + gg
+    int u, s, h;
+    int fresh;                 // k has moved since cv was loaded (an int: a bool costs byte moves in the loop)
+#ifdef PB_EXPERIMENT_PATH_STEPS
+    int steps;
+#endif
+    __device__ __forceinline__ void init(const uint32_t *tr_half, int end_j, int end_i, int pad, int hh, const uint32_t *hbuf,
+                                         const uint8_t *ad) {
+        const int q = max(end_i + pad - 1, 0), gg = q / R, r = q % R, t = end_j - 1 + gg;
+        h = hh;
+        base = reinterpret_cast<const uint4 *>(tr_half);
+        k = (t >> 2) * (WPS * 32) + gg;
+        u = t & 3; s = 28 - trace_shift<R>(h, r); fresh = 1;
+        hp = hbuf + end_j - 1; ap = ad + end_i - 1;
+        cv = make_uint4(0u, 0u, 0u, 0u);
+#ifdef PB_EXPERIMENT_PATH_STEPS
+        steps = 0;
+#endif
+    }
+    __device__ __forceinline__ uint32_t flags() {
+        if (fresh) { cv = base[k]; fresh = 0; }
+        const uint32_t lo = (u & 1) ? cv.y : cv.x, hi = (u & 1) ? cv.w : cv.z;
+        return (((u & 2) ? hi : lo) << s) >> 28;
+    }
+    __device__ __forceinline__ bool eq() { return ((*hp >> (8 + 16 * h)) & 0xFFu) == (uint32_t)__ldg(ap); }
+    __device__ __forceinline__ void move(bool consR, bool consA) {
+        const int s0 = 28 - trace_shift<R>(h, 0);
+        const bool wrap = consA && s == s0;
+        s = wrap ? s0 - 4 * (R - 1) : (consA ? s + 4 : s);
+        const int dt = (consR ? 1 : 0) + (wrap ? 1 : 0);
+        const bool back = u < dt;
+        u = (u - dt) & 3;
+        k -= (back ? WPS * 32 : 0) + (wrap ? 1 : 0);
+        fresh |= (back || wrap) ? 1 : 0;
+        if (consA) --ap;
+        if (consR) --hp;
+#ifdef PB_EXPERIMENT_PATH_STEPS
+        ++steps;
+#endif
+    }
+};
+
+#ifdef PB_EXPERIMENT_PATH_STEPS   // (measurement only: path steps of the traceback; tools/trace_path_steps.py)
+// [0] path steps, [1] traced alignments, [2] sum over warp slots of the longest path of the warp, [3] warp slots
+extern "C" { __device__ unsigned long long pb_path_stats[4]; }
+#endif
+
 // ---------------------------------------------------------------------------------------------------
 // trace_kernel: one group of G lanes per slot (two alignments in the s16x2 halves), 32/G slots per warp, R adapter
 // rows per lane (G*R >= adapter length; R = 5..8 so common adapter lengths 22/24/28 waste no rows).
@@ -331,6 +399,7 @@ trace_kernel(const TaskSrc ts, const uint8_t *__restrict__ seq,
     uint32_t *wsm = warp_smem + (size_t)warp * per_warp_words;
     uint32_t *hbuf = HBUF_SMEM ? (wsm + grp * max_n) : (gw + trace_words + (size_t)grp * max_n);
     ScoutCand *cand = reinterpret_cast<ScoutCand *>(wsm + hb_words);  // [half][lane]
+    TbTask *tbt = reinterpret_cast<TbTask *>(cand + 64) + grp * 2;    // [slot][half], this group's slot
     for (int64_t ws = wglobal; ws < n_wslots; ws += total_warps) {
         const int64_t slot = ws * SPW + grp;
         int nA, nB, mA, mB, nmax, nmin;
@@ -341,6 +410,14 @@ trace_kernel(const TaskSrc ts, const uint8_t *__restrict__ seq,
             const Task tA = get_task(ts, slot * 2);
             const Task tB = get_task(ts, slot * 2 + 1);
             nA = tA.n; nB = tB.n; mA = tA.m; mB = tB.m;
+            if (g < 2) {             // lane g traces half g
+                const Task &tk = g ? tB : tA;
+                TbTask b;
+                b.out_idx = tk.out_idx; b.flags = tk.flags | (tk.end_corr << 8); b.col0 = tk.col0; b.n_total = tk.n_total;
+                b.ad_off = tk.ad_off; b.end_j = tk.end_j; b.end_i = tk.end_i; b.end_score = tk.end_score;
+                b.n = tk.n; b.m = tk.m; b.pad0 = b.pad1 = 0;
+                tbt[g] = b;
+            }
             nmax = max(nA, nB);
             stage_columns<G>(hbuf, g, seq + tA.seq_off, nA, seq + tB.seq_off, nB, nmax, seq_ascii != 0, code_tab);
             lane_init<R>(L, g, G, sc, ads + tA.ad_off, mA, (tA.flags & TASK_LEFT_INF) != 0, ads + tB.ad_off, mB,
@@ -433,56 +510,46 @@ trace_kernel(const TaskSrc ts, const uint8_t *__restrict__ seq,
         cand[32 + lane] = make_cand<R>(L, 1, sc);
         __syncwarp();
 #ifndef PB_EXPERIMENT_SKIP_TRACEBACK   // (profiling experiments only: measure the forward pass alone)
+#ifdef PB_EXPERIMENT_PATH_STEPS
+        int path_steps = 0;
+#endif
         if (g < 2) {
             const int h = g;
-            const Task tk = get_task(ts, slot * 2 + h);
+            const TbTask tk = tbt[h];
             const HalfGeom gh = make_geom(tk.n, tk.m, G, R);
             if (tk.out_idx >= 0) {
                 EndCell end;
                 if (tk.flags & TASK_END_GIVEN) {
-                    end.j = tk.end_j; end.i = tk.end_i; end.score = tk.end_score; end.corr = tk.end_corr;
-                    if (tk.n_total <= 0 || tk.m <= 0) end.score = PB_SCORE_EMPTY;
+                    end.j = tk.end_j; end.i = tk.end_i; end.score = tk.end_score; end.corr = tk.flags >> 8;
+                    if (tk.n_total <= 0 || gh.m <= 0) end.score = PB_SCORE_EMPTY;
                 } else {
                     end = scout_combine(cand + h * 32 + grp * G, G, gh);
                 }
 #ifdef PB_EXPERIMENT_ALL_HOT   // the scout saw columns past the end: keep the traceback inside the matrix
-                end.j = min(end.j, tk.n); end.i = min(end.i, tk.m);
+                end.j = min(end.j, gh.n); end.i = min(end.i, gh.m);
 #endif
-                // cursor over the slot's trace: incremental addresses (lane of the row, row within the lane, step index) instead
-                // of a division per path step; one 128-bit load serves up to PB_TCHUNK consecutive steps of a lane
-                struct Cursor {
-                    const uint32_t *base;      // trace words of this half, lane 0 of the group, chunk 0
-                    const uint32_t *hp;        // staged column word of the current column
-                    const uint8_t *ap;         // adapter code of the current row
-                    int gg, r, t, key, h;
-                    uint4 cv;
-                    __device__ __forceinline__ uint32_t flags() {
-                        const int k = (t >> 2) * (WPS * 32) + gg;
-                        if (k != key) { cv = *reinterpret_cast<const uint4 *>(base + (size_t)k * PB_TCHUNK); key = k; }
-                        const uint32_t lo = (t & 1) ? cv.y : cv.x, hi = (t & 1) ? cv.w : cv.z;
-                        return (((t & 2) ? hi : lo) >> trace_shift<R>(h, r)) & 15u;
-                    }
-                    __device__ __forceinline__ bool eq() { return ((*hp >> (8 + 16 * h)) & 0xFFu) == (uint32_t)__ldg(ap); }
-                    __device__ __forceinline__ void move(bool consR, bool consA) {
-                        if (consA) { --ap; if (r == 0) { r = R - 1; --gg; --t; } else --r; }
-                        if (consR) { --t; --hp; }
-                    }
-                } cur;
-                {
-                    const int q = max(end.i + gh.pad - 1, 0);
-                    cur.gg = q / R; cur.r = q % R; cur.t = end.j - 1 + cur.gg; cur.key = -1; cur.h = h;
-                    cur.base = tr + ((size_t)trace_word<R>(h, 0) * 32 + grp * G) * PB_TCHUNK;
-                    cur.hp = hbuf + end.j - 1; cur.ap = ads + tk.ad_off + end.i - 1;
-                    cur.cv = make_uint4(0u, 0u, 0u, 0u);
-                }
+                TraceCursor<R, WPS> cur;
+                cur.init(tr + ((size_t)trace_word<R>(h, 0) * 32 + grp * G) * PB_TCHUNK, end.j, end.i, gh.pad, h, hbuf,
+                         ads + tk.ad_off);
                 int32_t rec[PB_REC];
-                int st = traceback_stats_cur(cur, end, sc.linear != 0, tk.col0, tk.n_total, tk.m, rec);
+                // matches from the score unless the scheme cannot tell a match from a mismatch by score
+                const int st = sc.ma != sc.mi ? traceback_stats_cur<true>(cur, end, sc.linear != 0, tk.col0, tk.n_total, gh.m, rec, &sc)
+                                              : traceback_stats_cur(cur, end, sc.linear != 0, tk.col0, tk.n_total, gh.m, rec);
                 if (st) atomicOr(status, 1);
                 int32_t *o = out + (size_t)tk.out_idx * PB_REC;
 #pragma unroll
                 for (int k = 0; k < PB_REC; ++k) __stcs(o + k, rec[k]);
+#ifdef PB_EXPERIMENT_PATH_STEPS
+                path_steps = cur.steps;
+                atomicAdd(&pb_path_stats[0], (unsigned long long)cur.steps);
+                atomicAdd(&pb_path_stats[1], 1ull);
+#endif
             }
         }
+#ifdef PB_EXPERIMENT_PATH_STEPS
+        path_steps = __reduce_max_sync(0xffffffffu, path_steps);
+        if (lane == 0) { atomicAdd(&pb_path_stats[2], (unsigned long long)path_steps); atomicAdd(&pb_path_stats[3], 1ull); }
+#endif
 #endif
         __syncwarp();
         // The slot's trace is dead now: drop its (dirty) L2 lines instead of letting them be written back to HBM
