@@ -209,6 +209,39 @@ int adapterTrimReads(const uint8_t *seqs, const int64_t *seq_off, int64_t n_seqs
 int adapterTrimReadsDevice(const uint8_t *d_seqs, const int64_t *d_seq_off, int64_t n_seqs, int64_t total_seq_bytes,
                            int64_t max_seq_len, const pb200_trim_args_t *args, int matchScore, int mismatchScore,
                            int gapOpenScore, int gapExtensionScore, void *stream);
+/* Porechop's output reads on the device: adapterTrimReadsDevice (same semantics, preconditions, stream and ordering rules, and
+ * host outputs), then the records get_fastq / get_fasta would write (porechop/nanopore_read.py:57-147) cut into caller-owned
+ * device buffers -- the records fastq.emit writes for these decisions, in the same order:
+ *   - a read without a middle hit: seq[start_trim : len - end_trim] (the whole read with `untrimmed`), if not empty;
+ *   - a read with hits: nothing with `discard_middle`, else the runs of its trimmed range outside the union of
+ *     [readStart - mid_extra_left[a], readEnd + 1 + mid_extra_right[a]) over its hits (clipped to the trimmed range), each
+ *     at least min_split_read_size long (get_split_read_parts), numbered 1, 2, ... in position order.
+ * Per record: bases (and qualities, from d_quals at the same offsets) copied as given -- no case or U/T change -- at
+ * d_out_off[r] .. d_out_off[r + 1]; d_out_read[r] = source read; d_out_part[r] = 0 (not split) or k >= 1 (the k-th part: the
+ * number add_number_to_read_name appends).  Records are in read order, the parts of a read in position order; names stay on
+ * the host.  Every record is a disjoint piece of its read, so total_seq_bytes bytes always suffice for d_out_seq / d_out_qual;
+ * the number of records is at most n_seqs + the number of hits.
+ * *n_parts and *n_out_bases are always written (0 on an argument error).  If *n_parts > parts_cap, or the hits do not fit
+ * hits_cap, the call returns PB200_ERR_SPACE: the host outputs and both totals are valid, the device outputs are not.  The
+ * call returns once the device outputs are written.
+ * Preconditions, checked before the device is touched (PB200_ERR_ARG otherwise): those of adapterTrimReadsDevice, split not
+ * NULL, parts_cap >= 0, both mid_extra_* arrays when n_mid_adapters > 0, d_out_qual NULL exactly when d_quals is NULL, and
+ * (n_seqs > 0) d_out_off, plus -- when parts_cap > 0 -- d_out_read / d_out_part and (total_seq_bytes > 0) d_out_seq.
+ * With no adapter on any side and no middle adapter every non-empty read comes out unchanged ("No adapters found"). */
+typedef struct {
+    const uint8_t *d_quals;            /* device, at the reads' offsets (quality length == read length), or NULL (FASTA) */
+    const int32_t *mid_extra_left;     /* host, per middle adapter: bases cut before a hit  (bad side if a start sequence) */
+    const int32_t *mid_extra_right;    /* host, per middle adapter: bases cut after a hit   (bad side if an end sequence)  */
+    int32_t min_split_read_size, discard_middle, untrimmed;
+    uint8_t *d_out_seq, *d_out_qual;   /* device, total_seq_bytes each (always enough); d_out_qual NULL iff d_quals NULL */
+    int64_t *d_out_off;                /* device, parts_cap + 1 */
+    int32_t *d_out_read, *d_out_part;  /* device, parts_cap */
+    int64_t parts_cap;
+    int64_t *n_parts, *n_out_bases;    /* host, always written */
+} pb200_split_args_t;
+int adapterTrimSplitReadsDevice(const uint8_t *d_seqs, const int64_t *d_seq_off, int64_t n_seqs, int64_t total_seq_bytes,
+                                int64_t max_seq_len, const pb200_trim_args_t *args, const pb200_split_args_t *split,
+                                int matchScore, int mismatchScore, int gapOpenScore, int gapExtensionScore, void *stream);
 /* cmin[l], l = 0 .. len-1: the smallest c with float("%f" % (100.0*c/l)) >= middle_threshold, or l+1 if none does
  * (cmin[0] = INT32_MAX).  The ">=" sibling of pb200TrimThresholdTable.  Pure host code; middle_threshold must be > 0. */
 int pb200MiddleThresholdTable(double middle_threshold, int32_t len, int32_t *cmin);

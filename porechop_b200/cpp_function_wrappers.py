@@ -98,6 +98,19 @@ C_LIB.adapterTrimReads.restype = c_int
 C_LIB.adapterTrimReadsDevice.argtypes = [c_void_p, c_void_p, c_int64, c_int64, c_int64, POINTER(TrimArgsDesc), c_int, c_int,
                                          c_int, c_int, c_void_p]
 C_LIB.adapterTrimReadsDevice.restype = c_int
+
+
+class SplitArgsDesc(Structure):
+    """pb200_split_args_t (include/porechop_b200.h)"""
+    _fields_ = [('d_quals', c_void_p), ('mid_extra_left', c_void_p), ('mid_extra_right', c_void_p),
+                ('min_split_read_size', c_int32), ('discard_middle', c_int32), ('untrimmed', c_int32),
+                ('d_out_seq', c_void_p), ('d_out_qual', c_void_p), ('d_out_off', c_void_p), ('d_out_read', c_void_p),
+                ('d_out_part', c_void_p), ('parts_cap', c_int64), ('n_parts', c_void_p), ('n_out_bases', c_void_p)]
+
+
+C_LIB.adapterTrimSplitReadsDevice.argtypes = [c_void_p, c_void_p, c_int64, c_int64, c_int64, POINTER(TrimArgsDesc),
+                                              POINTER(SplitArgsDesc), c_int, c_int, c_int, c_int, c_void_p]
+C_LIB.adapterTrimSplitReadsDevice.restype = c_int
 C_LIB.pb200MiddleThresholdTable.argtypes = [c_double, c_int32, c_void_p]
 C_LIB.pb200MiddleThresholdTable.restype = c_int
 C_LIB.pb200FormatRecord.argtypes = [c_void_p, c_char_p, c_int]
@@ -123,7 +136,7 @@ EXPORTED_SYMBOLS = ['adapterAlignment', 'freeCString', 'adapterAlignmentBatch', 
                     'adapterAlignmentBatchDevice', 'adapterEndDecisions', 'pb200TrimThresholdTable', 'adapterSetSearch',
                     'adapterMiddleScan',
                     'adapterMiddleScanDevice', 'pb200MiddleThresholdTable', 'adapterTrimReads', 'adapterTrimReadsDevice',
-                    'pb200FormatRecord', 'pb200DeviceCount', 'pb200SetDevice', 'pb200Synchronize', 'pb200LastError',
+                    'adapterTrimSplitReadsDevice', 'pb200FormatRecord', 'pb200DeviceCount', 'pb200SetDevice', 'pb200Synchronize', 'pb200LastError',
                     'pb200KernelLaunches', 'pb200TimingEnable', 'pb200TimingRead', 'pb200TimingReadKinds', 'pb200SetOption',
                     'pb200GetOption', 'pb200HostBuffer', 'pb200PackNibbles']
 
@@ -452,6 +465,41 @@ def adapter_trim_reads_device(d_seqs_ptr, d_seq_off_ptr, n_seqs, total_seq_bytes
         c_void_p(d_seqs_ptr), c_void_p(d_seq_off_ptr), n_seqs, total_seq_bytes, max_seq_len, args, ma, mi, go, ge,
         c_void_p(stream_ptr)), int(n_seqs), start, end, middle, end_size, extra_trim_size, end_threshold, min_trim_size,
         middle_threshold, want_top2)
+
+
+def adapter_trim_split_reads_device(d_seqs_ptr, d_seq_off_ptr, n_seqs, total_seq_bytes, max_seq_len, start, end, middle,
+                                    scoring_scheme_vals, end_size, extra_trim_size, end_threshold, min_trim_size,
+                                    middle_threshold=85.0, want_top2=False, stream_ptr=0, *, d_quals_ptr=0, mid_extra=None,
+                                    min_split_read_size=1000, discard_middle=False, untrimmed=False, d_out_seq_ptr=0,
+                                    d_out_qual_ptr=0, d_out_off_ptr=0, d_out_read_ptr=0, d_out_part_ptr=0, parts_cap=0):
+    """adapter_trim_reads_device, then Porechop's output records cut into caller-owned device buffers
+    (adapterTrimSplitReadsDevice): bases (d_out_seq), qualities (d_out_qual, when d_quals is given), offsets int64[parts_cap + 1],
+    source read and part number int32[parts_cap] (0 = not split, k >= 1 = the k-th part).  mid_extra: (left, right) per middle
+    adapter -- the bases cut before and after a hit (None when there are no middle adapters).
+    Returns the outputs of adapter_trim_reads_device plus (n_parts, n_out_bases).  When the records do not fit parts_cap it
+    raises EngineError with code ERR_SPACE and the totals as .n_parts / .n_out_bases: the buffers are the caller's, so the
+    caller allocates them again and repeats the call."""
+    ma, mi, go, ge = [int(x) for x in scoring_scheme_vals]
+    n_mid = len(middle[1]) - 1 if middle is not None else 0
+    left, right = mid_extra if mid_extra is not None else ([], [])
+    left = np.ascontiguousarray(left, dtype=np.int32)
+    right = np.ascontiguousarray(right, dtype=np.int32)
+    if len(left) != n_mid or len(right) != n_mid:
+        raise ValueError('mid_extra needs one (left, right) value per middle adapter')
+    n_parts, n_bases = c_int64(0), c_int64(0)
+    split = SplitArgsDesc(d_quals_ptr or None, left.ctypes.data if n_mid else None, right.ctypes.data if n_mid else None,
+                          int(min_split_read_size), int(bool(discard_middle)), int(bool(untrimmed)), d_out_seq_ptr or None,
+                          d_out_qual_ptr or None, d_out_off_ptr or None, d_out_read_ptr or None, d_out_part_ptr or None,
+                          int(parts_cap), addressof(n_parts), addressof(n_bases))
+    try:
+        out = _trim_reads(lambda args: C_LIB.adapterTrimSplitReadsDevice(
+            c_void_p(d_seqs_ptr), c_void_p(d_seq_off_ptr), n_seqs, total_seq_bytes, max_seq_len, args, byref(split), ma, mi, go,
+            ge, c_void_p(stream_ptr)), int(n_seqs), start, end, middle, end_size, extra_trim_size, end_threshold, min_trim_size,
+            middle_threshold, want_top2)
+    except EngineError as e:
+        e.n_parts, e.n_out_bases = n_parts.value, n_bases.value
+        raise
+    return out + (n_parts.value, n_bases.value)
 
 
 def middle_threshold_table(middle_threshold, length):

@@ -701,4 +701,24 @@ PB_HD uint32_t score_pair(const int32_t *r, int *overflow) {
     return (uint32_t)r[7] | ((uint32_t)r[8] << 16);
 }
 
+// Split rule of the output stage (adapterTrimSplitReadsDevice): get_split_read_parts (nanopore_read.py:76-95) on a trimmed
+// read of `len` bases.  The kept parts are the runs of [0, len) outside every range [rng[2k], rng[2k + 1]) -- clipped to the
+// read, empty ones ignored -- that are at least min_size long (and never empty).  The ranges come sorted by start, so one sweep
+// over them finds the union.  f(k, start, end) is called for the k-th kept part (k = 0, 1, ...); returns their number.
+template <class F>
+PB_HD int64_t split_runs(int64_t len, const int32_t *rng, int32_t n_rng, int64_t min_size, F &&f) {
+    int64_t cur = 0, k = 0;
+    for (int32_t r = 0; r <= n_rng; ++r) {
+        int64_t x = len, y = len;                 // r == n_rng: the run up to the end of the read
+        if (r < n_rng) {
+            x = rng[2 * r] > 0 ? rng[2 * r] : 0;
+            y = rng[2 * r + 1] < len ? rng[2 * r + 1] : len;
+            if (y <= x) continue;
+        }
+        if (x > cur && x - cur >= min_size) f(k++, cur, x);
+        if (y > cur) cur = y;
+    }
+    return k;
+}
+
 }  // namespace pb

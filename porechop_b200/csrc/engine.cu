@@ -194,6 +194,9 @@ struct Engine {
     // whole-read trimming (adapterTrimReads*): the segment's ASCII reads and offsets (host API), window offsets, start / end
     // windows, segment-wide start / end trims, the first base of every trimmed read, tile sums of the offset scans
     DevBuf trim_reads, trim_off, trim_win_off, trim_win[2], trim_d[2], trim_first, trim_scan;
+    // output stage (adapterTrimSplitReadsDevice): the segment's hit reads, their CSR of extended hit ranges, hit row per read,
+    // records and bases per read (scanned in place), source offset per record
+    DevBuf split_hits, split_rng_off, split_rng, split_hit_of, split_cnt, split_bytes, split_src;
     // adapter-set search (adapterSetSearch): NSTAGE slices of search_cols u64 keys, one per stage, so that stages running at
     // once never share an accumulator; a batch owns the columns [search_col, search_col + n_adapters) of every slice
     DevBuf search_acc;
@@ -1892,10 +1895,14 @@ int trim_side_check(const pb200_trim_side_t &T, int64_t n_seqs, int32_t end_size
 // The reads [a, b) of the next segment: the middle scan's budget (middle_segment_end) with, per read, the two end windows (and
 // their codes when they are encoded), window offsets, two trims, the trimmed range's first base and -- host API -- the
 // segment's ASCII reads and offsets next to their codes.
-int64_t trim_segment_end(const Engine &E, int64_t a, int64_t n_seqs, int32_t n_mid, int64_t wl_max, const int64_t *h_seq_off) {
-    const size_t held = E.trim_reads.cap + E.trim_off.cap + E.trim_win_off.cap + E.trim_win[0].cap + E.trim_win[1].cap +
-                        E.trim_d[0].cap + E.trim_d[1].cap + E.trim_first.cap;
-    int64_t b = middle_segment_end(E, a, n_seqs, n_mid, h_seq_off, 3.0 * (double)wl_max + 40, h_seq_off ? 2.0 : 1.0, held);
+// split: the output stage's buffers too (hit row, records and bases per read, the source offset of up to two records per read).
+int64_t trim_segment_end(const Engine &E, int64_t a, int64_t n_seqs, int32_t n_mid, int64_t wl_max, const int64_t *h_seq_off,
+                         bool split = false) {
+    size_t held = E.trim_reads.cap + E.trim_off.cap + E.trim_win_off.cap + E.trim_win[0].cap + E.trim_win[1].cap +
+                  E.trim_d[0].cap + E.trim_d[1].cap + E.trim_first.cap;
+    if (split) held += E.split_hit_of.cap + E.split_cnt.cap + E.split_bytes.cap + E.split_src.cap;
+    int64_t b = middle_segment_end(E, a, n_seqs, n_mid, h_seq_off, 3.0 * (double)wl_max + 40 + (split ? 44.0 : 0.0),
+                                   h_seq_off ? 2.0 : 1.0, held);
 #ifdef PB_TEST_SEGMENT_READS
     // tests of the host-simulated engine only (through sim_engine.load): small segments, so that a few reads span several
     b = std::min<int64_t>(b, a + PB_TEST_SEGMENT_READS);
@@ -1903,9 +1910,102 @@ int64_t trim_segment_end(const Engine &E, int64_t a, int64_t n_seqs, int32_t n_m
     return b;
 }
 
+// Output stage of adapterTrimSplitReadsDevice: the running totals over the segments, and whether the records still fit parts_cap
+// (once they do not, the stage only counts).
+struct SplitTotals { int64_t parts = 0, bases = 0; bool write = true; };
+
+// One segment's records [a, a + n): reads at reads[off[s] ..], trimmed ranges first[s] / toff (scanned lengths) on the device;
+// the segment's hits are the rounds from rounds[r0] on (segment-relative reads, {adapter, record} each).
+int split_segment(Engine &E, cudaStream_t stream, const pb200_split_args_t &X, const uint8_t *reads, const int64_t *off, int64_t a,
+                  int64_t n, const int64_t *first, const int64_t *toff, const std::vector<MiddleRound> &rounds, size_t r0,
+                  SplitTotals &T) {
+    // ---- the hit reads and their extended ranges (rs - left, re + right) sorted by start: a CSR, a few ints per hit ----
+    struct Rng { int32_t read, x, y; };
+    std::vector<Rng> all;
+    for (size_t k = r0; k < rounds.size(); ++k) {
+        const MiddleRound &R = rounds[k];
+        for (size_t p = 0; p < R.reads.size(); ++p) {
+            const int32_t *h = R.hits.data() + p * PB_HIT_INTS;
+            const auto clamp = [](int64_t v) { return (int32_t)std::min<int64_t>(std::max<int64_t>(v, INT32_MIN), INT32_MAX); };
+            // record ends are inclusive: the reference masks and trims up to readEnd + 1
+            all.push_back(Rng{R.reads[p], clamp((int64_t)h[1] - X.mid_extra_left[h[0]]),
+                              clamp((int64_t)h[2] + 1 + X.mid_extra_right[h[0]])});
+        }
+    }
+    std::sort(all.begin(), all.end(), [](const Rng &u, const Rng &v) { return u.read != v.read ? u.read < v.read : u.x < v.x; });
+    std::vector<int32_t> hit_reads, rng_off(1, 0), rng;
+    rng.reserve(all.size() * 2);
+    for (size_t k = 0; k < all.size(); ++k) {
+        if (k == 0 || all[k].read != all[k - 1].read) {
+            if (k) rng_off.push_back((int32_t)k);
+            hit_reads.push_back(all[k].read);
+        }
+        rng.push_back(all[k].x);
+        rng.push_back(all[k].y);
+    }
+    if (!all.empty()) rng_off.push_back((int32_t)all.size());
+    const int64_t n_h = (int64_t)hit_reads.size();
+    if (int rc = E.split_hit_of.ensure((size_t)n * 4 + 16)) return rc;
+    if (int rc = E.split_hits.ensure((size_t)n_h * 4 + 16)) return rc;
+    if (int rc = E.split_rng_off.ensure((size_t)(n_h + 1) * 4 + 16)) return rc;
+    if (int rc = E.split_rng.ensure(rng.size() * 4 + 16)) return rc;
+    if (int rc = E.split_cnt.ensure((size_t)(n + 1) * 8)) return rc;
+    if (int rc = E.split_bytes.ensure((size_t)(n + 1) * 8)) return rc;
+    CK(cudaMemsetAsync(E.split_hit_of.p, 0xFF, (size_t)n * 4, stream));
+    if (n_h) {
+        CK(cudaMemcpyAsync(E.split_hits.p, hit_reads.data(), (size_t)n_h * 4, cudaMemcpyHostToDevice, stream));
+        CK(cudaMemcpyAsync(E.split_rng_off.p, rng_off.data(), (size_t)(n_h + 1) * 4, cudaMemcpyHostToDevice, stream));
+        CK(cudaMemcpyAsync(E.split_rng.p, rng.data(), rng.size() * 4, cudaMemcpyHostToDevice, stream));
+        split_mark_kernel<<<(unsigned)((n_h + 255) / 256), 256, 0, stream>>>(static_cast<const int32_t *>(E.split_hits.as<int32_t>()),
+                                                                             n_h, E.split_hit_of.as<int32_t>());
+        g_launches++;
+    }
+    // the segment as the output stage's kernels read it (PB_SPLIT_READS_PARAMS)
+    const int32_t *hit_of = E.split_hit_of.as<int32_t>(), *rng_off_d = E.split_rng_off.as<int32_t>(),
+                  *rng_d = E.split_rng.as<int32_t>();
+    const int64_t min_split = X.min_split_read_size;
+    // ---- records and bases per read, scanned; the segment's totals come home ----
+    int64_t *cnt = E.split_cnt.as<int64_t>(), *bytes = E.split_bytes.as<int64_t>();
+    split_count_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(off, first, toff, hit_of, rng_off_d, rng_d, n, min_split,
+                                                                        X.discard_middle, X.untrimmed, cnt, bytes);
+    g_launches++;
+    CK(cudaGetLastError());
+    if (int rc = scan_offsets(E, stream, cnt, n)) return rc;
+    if (int rc = scan_offsets(E, stream, bytes, n)) return rc;
+    int64_t seg[2] = {0, 0};
+    CK(cudaMemcpyAsync(&seg[0], cnt + n, 8, cudaMemcpyDeviceToHost, stream));
+    CK(cudaMemcpyAsync(&seg[1], bytes + n, 8, cudaMemcpyDeviceToHost, stream));
+    CK(cudaStreamSynchronize(stream));
+    if (T.write && T.parts + seg[0] > X.parts_cap) T.write = false;     // PB200_ERR_SPACE: from here on only count
+    if (T.write) {
+        // ---- each record's output offset, read, part and source; then the gather, one warp per record ----
+        if (int rc = E.split_src.ensure((size_t)seg[0] * 8 + 16)) return rc;
+        int64_t *src = E.split_src.as<int64_t>();
+        split_write_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(off, first, toff, hit_of, rng_off_d, rng_d, n, min_split,
+                                                                            X.discard_middle, X.untrimmed,
+                                                                            static_cast<const int64_t *>(cnt),
+                                                                            static_cast<const int64_t *>(bytes), T.parts, T.bases, a,
+                                                                            src, X.d_out_off, X.d_out_read, X.d_out_part);
+        g_launches++;
+        if (seg[0] > 0) {
+            const int64_t blocks = std::max<int64_t>(1, std::min<int64_t>((seg[0] + 7) / 8, (int64_t)E.sm_count * 8));
+            split_gather_kernel<<<(unsigned)blocks, 256, 0, stream>>>(reads, X.d_quals, static_cast<const int64_t *>(src),
+                                                                      static_cast<const int64_t *>(X.d_out_off + T.parts), seg[0],
+                                                                      X.d_out_seq, X.d_out_qual);
+            g_launches++;
+        }
+        CK(cudaGetLastError());
+    }
+    T.parts += seg[0];
+    T.bases += seg[1];
+    return 0;
+}
+
 // device: seqs / seq_off are device pointers (adapterTrimReadsDevice), else host buffers uploaded segment by segment.
+// X: the output stage of adapterTrimSplitReadsDevice (device reads only), or nullptr.
 int trim_reads(const uint8_t *seqs, const int64_t *seq_off, int64_t n_seqs, bool device, int64_t total_seq_bytes,
-               int64_t max_seq_len, const pb200_trim_args_t *A, int ma, int mi, int go, int ge, void *user_stream) {
+               int64_t max_seq_len, const pb200_trim_args_t *A, int ma, int mi, int go, int ge, void *user_stream,
+               const pb200_split_args_t *X = nullptr) {
     // ---- preconditions: nothing below touches the device before they all hold ----
     if (!A) return fail(PB200_ERR_ARG, "NULL pointer");
     if (n_seqs < 0 || total_seq_bytes < 0) return fail(PB200_ERR_ARG, "negative count");
@@ -1938,6 +2038,16 @@ int trim_reads(const uint8_t *seqs, const int64_t *seq_off, int64_t n_seqs, bool
         }
     }
     if (max_len > 0x7fff0000ll) return fail(PB200_ERR_ARG, "sequence longer than 2^31");
+    if (X) {
+        if (!device) return fail(PB200_ERR_ARG, "the output stage takes device reads only");
+        if (X->parts_cap < 0) return fail(PB200_ERR_ARG, "negative count");
+        if (!X->n_parts || !X->n_out_bases) return fail(PB200_ERR_ARG, "NULL pointer");
+        if (n_mid > 0 && (!X->mid_extra_left || !X->mid_extra_right)) return fail(PB200_ERR_ARG, "NULL pointer");
+        if (!X->d_quals != !X->d_out_qual) return fail(PB200_ERR_ARG, "d_out_qual must be NULL exactly when d_quals is NULL");
+        if (n_seqs > 0 && (!X->d_out_off || (X->parts_cap > 0 && (!X->d_out_read || !X->d_out_part ||
+                                                                  (total_seq_bytes > 0 && !X->d_out_seq)))))
+            return fail(PB200_ERR_ARG, "NULL pointer");
+    }
     if (A->n_hits && n_seqs > 0) memset(A->n_hits, 0, (size_t)n_seqs * 4);
     if (A->n_total) *A->n_total = 0;
     for (int k = 0; k < 2; ++k) {         // a side without adapters: nothing aligns, nothing is trimmed
@@ -1946,7 +2056,8 @@ int trim_reads(const uint8_t *seqs, const int64_t *seq_off, int64_t n_seqs, bool
         memset(T.trim, 0, (size_t)n_seqs * 4);
         if (T.top2) for (int64_t s = 0; s < n_seqs; ++s) { int32_t *o = T.top2 + s * 6; o[0] = o[3] = -1; o[1] = o[4] = 0; o[2] = o[5] = 1; }
     }
-    if (n_seqs == 0 || (A->start.n_adapters == 0 && A->end.n_adapters == 0 && n_mid == 0)) return 0;
+    // without adapters nothing is trimmed or split; the output stage still writes every non-empty read ("No adapters found")
+    if (n_seqs == 0 || (!X && A->start.n_adapters == 0 && A->end.n_adapters == 0 && n_mid == 0)) return 0;
 
     Engine *Ep = nullptr;
     if (int rc = get_engine(&Ep)) return rc;
@@ -1957,8 +2068,9 @@ int trim_reads(const uint8_t *seqs, const int64_t *seq_off, int64_t n_seqs, bool
     cudaStream_t stream = S.stream;
     if (device) { if (int rc = library_stream(E, user_stream, &stream)) return rc; }
     if (int rc = order_after_last(E, stream)) return rc;
-    NvtxRange submit_range("pb200:submit_trim");
+    NvtxRange submit_range(X ? "pb200:submit_trim_split" : "pb200:submit_trim");
     std::vector<MiddleRound> rounds;
+    SplitTotals totals;
     auto run = [&]() -> int {
         if (int rc = reset_misc(S, stream)) return rc;
         if (int rc = check_status(S, stream)) return rc;     // a deferred error of an earlier device-resident call
@@ -1987,7 +2099,7 @@ int trim_reads(const uint8_t *seqs, const int64_t *seq_off, int64_t n_seqs, bool
             if (int rc = E.mid_codes.ensure((size_t)total_seq_bytes + 16)) return rc;
         }
         for (int64_t a = 0; a < n_seqs;) {
-            const int64_t b = trim_segment_end(E, a, n_seqs, n_mid, wl_max, device ? nullptr : seq_off);
+            const int64_t b = trim_segment_end(E, a, n_seqs, n_mid, wl_max, device ? nullptr : seq_off, X != nullptr);
             const int64_t n = b - a;
             // the segment's reads: ASCII at reads[off[s] .. off[s+1])
             const uint8_t *reads = seqs;
@@ -2057,6 +2169,18 @@ int trim_reads(const uint8_t *seqs, const int64_t *seq_off, int64_t n_seqs, bool
             }
             if (n_mid == 0) {
                 if (int rc = check_status(S, stream)) return rc;
+                if (X) {                     // the trimmed ranges the middle scan would have made, then the output stage
+                    if (int rc = E.trim_first.ensure((size_t)n * 8 + 16)) return rc;
+                    if (int rc = E.mid_off.ensure((size_t)(n + 1) * 8)) return rc;
+                    int64_t *toff = E.mid_off.as<int64_t>();
+                    trimmed_range_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(
+                        off, static_cast<const int32_t *>(E.trim_d[0].as<int32_t>()), static_cast<const int32_t *>(E.trim_d[1].as<int32_t>()),
+                        n, E.trim_first.as<int64_t>(), toff);
+                    g_launches++;
+                    if (int rc = scan_offsets(E, stream, toff, n)) return rc;
+                    if (int rc = split_segment(E, stream, *X, reads, off, a, n, E.trim_first.as<int64_t>(), toff, rounds, rounds.size(),
+                                               totals)) return rc;
+                }
                 a = b;
                 continue;
             }
@@ -2086,9 +2210,15 @@ int trim_reads(const uint8_t *seqs, const int64_t *seq_off, int64_t n_seqs, bool
                                              M.rec + (size_t)c0 * n_mid * PB_REC, nullptr, 0, A->mid_ad_off)) return rc;
                 if (int rc = launch_middle_decide(E, stream, M, n_mid, nullptr, c0, cnt, M.active[0], S.misc.as<int>())) return rc;
             }
+            const size_t r0 = rounds.size();
             if (int rc = middle_rounds(E, S, stream, PM, M, n_mid, A->mid_ad_off, a, rounds)) return rc;
+            if (X) {
+                if (int rc = split_segment(E, stream, *X, reads, off, a, n, E.trim_first.as<int64_t>(), M.off, rounds, r0, totals))
+                    return rc;
+            }
             a = b;
         }
+        if (X) CK(cudaStreamSynchronize(stream));      // the device outputs are written when the call returns
         return 0;
     };
     const int rc = run();
@@ -2098,8 +2228,13 @@ int trim_reads(const uint8_t *seqs, const int64_t *seq_off, int64_t n_seqs, bool
         g_err = first_err;
     }
     E.last_pending = false;               // the stream waited for an earlier call's queued work, and all of it is done
-    if (rc || n_mid == 0) return rc;
-    return middle_emit(rounds, n_seqs, A->n_hits, A->hits, A->hits_cap, A->n_total);
+    if (X && !rc) { *X->n_parts = totals.parts; *X->n_out_bases = totals.bases; }
+    if (rc) return rc;
+    if (n_mid > 0) {
+        if (int rc2 = middle_emit(rounds, n_seqs, A->n_hits, A->hits, A->hits_cap, A->n_total)) return rc2;
+    }
+    if (X && totals.parts > X->parts_cap) return fail(PB200_ERR_SPACE, "parts_cap is smaller than the number of records (*n_parts)");
+    return 0;
 }
 
 }  // namespace
@@ -2162,6 +2297,16 @@ int adapterTrimReadsDevice(const uint8_t *d_seqs, const int64_t *d_seq_off, int6
                            int64_t max_seq_len, const pb200_trim_args_t *args, int ma, int mi, int go, int ge, void *stream) {
     g_err.clear();
     return trim_reads(d_seqs, d_seq_off, n_seqs, true, total_seq_bytes, max_seq_len, args, ma, mi, go, ge, stream);
+}
+
+int adapterTrimSplitReadsDevice(const uint8_t *d_seqs, const int64_t *d_seq_off, int64_t n_seqs, int64_t total_seq_bytes,
+                                int64_t max_seq_len, const pb200_trim_args_t *args, const pb200_split_args_t *split, int ma, int mi,
+                                int go, int ge, void *stream) {
+    g_err.clear();
+    if (!split) return fail(PB200_ERR_ARG, "NULL pointer");
+    if (split->n_parts) *split->n_parts = 0;
+    if (split->n_out_bases) *split->n_out_bases = 0;
+    return trim_reads(d_seqs, d_seq_off, n_seqs, true, total_seq_bytes, max_seq_len, args, ma, mi, go, ge, stream, split);
 }
 
 int pb200MiddleThresholdTable(double middle_threshold, int32_t len, int32_t *cmin) {

@@ -11,6 +11,8 @@
 //   middle_decide_kernel one round of the middle-adapter scan: first hit per active read, masking, next active list
 //   window_len / cut_windows / trimmed_range / gather_encode + scan_*: whole-read trimming (adapterTrimReads) -- end windows
 //                        cut from resident reads, trims turned into the trimmed reads the middle scan masks
+//   split_mark / split_count / split_write / split_gather: output stage of adapterTrimSplitReadsDevice -- Porechop's output
+//                        records counted, placed and gathered (bases + qualities) into the caller's buffers
 //   generic_kernel       int32 thread-serial fallback for scoring schemes / adapters outside the int16 domain
 //
 // The arithmetic is in dp_core.cuh (shared with the CPU emulation used by the tests).
@@ -1140,6 +1142,128 @@ __global__ void gather_encode_kernel(const uint8_t *reads, const int64_t *off, c
         const uint8_t *src = reads + off[s] + first[s];
         const int64_t d0 = dst_off[s], len = dst_off[s + 1] - d0;
         for (int64_t k = lane; k < len; k += 32) codes[d0 + k] = (uint8_t)encode_byte(src[k]);
+    }
+}
+
+// ---------------------------------------------------------------------------------------------------
+// Output stage of adapterTrimSplitReadsDevice, once per segment: the records Porechop writes (get_fastq / get_fasta) cut from
+// the caller's reads.  Count records and bases per read, scan both, write each record's source, part number and output
+// offset, then gather the bases (and qualities) into the caller's output buffers.
+//
+// What the segment's reads look like to the stage (all read only): reads at off[s] .. off[s+1]; the trimmed range starts at
+// first[s] and is toff[s+1] - toff[s] long; hit_of[s] = -1 for a read without a middle hit, else its row of the CSR
+// rng_off / rng of extended hit ranges (trimmed-read coordinates, sorted by start).  The kernels take these as plain pointer
+// arguments (so that each is an access of its own, read because it is const) and assemble the view below themselves.
+#define PB_SPLIT_READS_PARAMS const int64_t *off, const int64_t *first, const int64_t *toff, const int32_t *hit_of, \
+                              const int32_t *rng_off, const int32_t *rng, int64_t n, int64_t min_split, int32_t discard_middle, \
+                              int32_t untrimmed
+#define PB_SPLIT_READS_VIEW {off, first, toff, hit_of, rng_off, rng, n, min_split, discard_middle, untrimmed}
+struct SplitReads {
+    const int64_t *off, *first, *toff;
+    const int32_t *hit_of, *rng_off, *rng;
+    int64_t n, min_split;
+    int32_t discard_middle, untrimmed;
+};
+// the output records of read s: f(part, source offset, length) in position order; returns their number
+template <class F>
+__device__ __forceinline__ int64_t read_records(const SplitReads &r, int64_t s, F &&f) {
+    const int64_t base = r.off[s], a = r.first[s], tl = r.toff[s + 1] - r.toff[s];
+    const int32_t h = r.hit_of[s];
+    if (h < 0) {                                  // not split: the trimmed read (the whole read with --untrimmed), if not empty
+        const int64_t l = r.untrimmed ? r.off[s + 1] - base : tl;
+        if (l <= 0) return 0;
+        f(0, r.untrimmed ? base : base + a, l);
+        return 1;
+    }
+    if (r.discard_middle) return 0;
+    const int32_t k0 = r.rng_off[h];
+    return split_runs(tl, r.rng + 2 * (int64_t)k0, r.rng_off[h + 1] - k0, r.min_split,
+                      [&](int64_t k, int64_t x, int64_t y) { f(k + 1, base + a + x, y - x); });
+}
+// hit_of[hit_reads[i]] = i (hit_of was set to -1)
+__global__ void split_mark_kernel(const int32_t *hit_reads, int64_t n_hit_reads, int32_t *hit_of) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n_hit_reads) hit_of[hit_reads[i]] = (int32_t)i;
+}
+// records and bases of every read -> cnt[s + 1], bytes[s + 1] (cnt[0] = bytes[0] = 0), for scan_offsets
+__global__ void split_count_kernel(PB_SPLIT_READS_PARAMS, int64_t *cnt, int64_t *bytes) {
+    const SplitReads r = PB_SPLIT_READS_VIEW;
+    const int64_t s = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (s == 0) { cnt[0] = 0; bytes[0] = 0; }
+    if (s >= r.n) return;
+    int64_t b = 0;
+    cnt[s + 1] = read_records(r, s, [&](int64_t, int64_t, int64_t l) { b += l; });
+    bytes[s + 1] = b;
+}
+// the records of the segment from the scanned counts: record rec0 + rec_off[s] + j of read read0 + s gets its output offset
+// byte0 + ..., read, part and (segment-relative record index) source offset; thread 0 also writes the offset after the
+// segment's last record
+__global__ void split_write_kernel(PB_SPLIT_READS_PARAMS, const int64_t *rec_off, const int64_t *byte_off, int64_t rec0,
+                                   int64_t byte0, int64_t read0, int64_t *src, int64_t *out_off, int32_t *out_read,
+                                   int32_t *out_part) {
+    const SplitReads r = PB_SPLIT_READS_VIEW;
+    const int64_t s = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (s == 0) out_off[rec0 + rec_off[r.n]] = byte0 + byte_off[r.n];
+    if (s >= r.n) return;
+    int64_t i = rec_off[s], pos = byte0 + byte_off[s];
+    read_records(r, s, [&](int64_t part, int64_t from, int64_t l) {
+        out_off[rec0 + i] = pos;
+        out_read[rec0 + i] = (int32_t)(read0 + s);
+        out_part[rec0 + i] = (int32_t)part;
+        src[i] = from;
+        ++i;
+        pos += l;
+    });
+}
+// dst[0 .. n) = src[0 .. n) by one warp: the bytes up to dst's next 16-byte boundary one per lane, then aligned 16-byte stores
+// assembled from aligned 16-byte loads (each lane's chunk and the next lane's, shifted into place with __funnelshift_r), then
+// the last bytes one per lane.  Loads never leave [src & ~15, src + n): the body stops where its next chunk would.
+__device__ __forceinline__ void warp_copy(const uint8_t *src, uint8_t *dst, int64_t n, int lane) {
+    int64_t h = (int64_t)((16 - ((uintptr_t)dst & 15)) & 15);
+    if (h > n) h = n;
+    if (lane < h) dst[lane] = src[lane];
+    const uintptr_t s1 = (uintptr_t)(src + h);
+    const uint4 *A = reinterpret_cast<const uint4 *>(s1 & ~(uintptr_t)15);
+    const int o = (int)(s1 & 15), q = o >> 2;
+    const unsigned sh = (unsigned)(o & 3) * 8;
+    const int64_t rem = n - h;
+    int64_t nvec = o ? ((rem + o) >> 4) - 1 : rem >> 4;     // 16-byte stores; their chunks (+ the next one if o > 0) fit
+    if (nvec < 0) nvec = 0;
+    const int64_t nchunk = nvec + (o ? 1 : 0);
+    uint4 *D = reinterpret_cast<uint4 *>(dst + h);
+    for (int64_t v0 = 0; v0 < nvec; v0 += 32) {              // warp-uniform trip count
+        const int64_t v = v0 + lane;
+        const uint4 c = v < nchunk ? A[v] : make_uint4(0u, 0u, 0u, 0u);
+        uint4 d;
+        d.x = __shfl_sync(0xffffffffu, c.x, (lane + 1) & 31);
+        d.y = __shfl_sync(0xffffffffu, c.y, (lane + 1) & 31);
+        d.z = __shfl_sync(0xffffffffu, c.z, (lane + 1) & 31);
+        d.w = __shfl_sync(0xffffffffu, c.w, (lane + 1) & 31);
+        if (lane == 31 && v + 1 < nchunk) d = A[v + 1];
+        // words o/4 .. o/4 + 4 of the 32 bytes c:d, then shifted right by (o & 3) bytes
+        const bool q2 = q & 2, q1 = q & 1;
+        const unsigned t0 = q2 ? c.z : c.x, t1 = q2 ? c.w : c.y, t2 = q2 ? d.x : c.z, t3 = q2 ? d.y : c.w, t4 = q2 ? d.z : d.x,
+                       t5 = q2 ? d.w : d.y;
+        const unsigned u0 = q1 ? t1 : t0, u1 = q1 ? t2 : t1, u2 = q1 ? t3 : t2, u3 = q1 ? t4 : t3, u4 = q1 ? t5 : t4;
+        if (v < nvec)
+            D[v] = make_uint4(__funnelshift_r(u0, u1, sh), __funnelshift_r(u1, u2, sh), __funnelshift_r(u2, u3, sh),
+                              __funnelshift_r(u3, u4, sh));
+    }
+    const int64_t t = h + 16 * nvec;                         // at most 30 bytes are left
+    if (lane < n - t) dst[t + lane] = src[t + lane];
+}
+// bases (and qualities) of records [0, n_rec) of the segment: source src[i], output out_off[i] .. out_off[i + 1] (out_off = the
+// caller's offsets from the segment's first record on); one warp per record
+__global__ void __launch_bounds__(256) split_gather_kernel(const uint8_t *__restrict__ seq, const uint8_t *__restrict__ qual,
+                                                           const int64_t *__restrict__ src, const int64_t *__restrict__ out_off,
+                                                           int64_t n_rec, uint8_t *__restrict__ out_seq,
+                                                           uint8_t *__restrict__ out_qual) {
+    const int lane = threadIdx.x & 31;
+    const int64_t warps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    for (int64_t i = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < n_rec; i += warps) {
+        const int64_t from = src[i], to = out_off[i], len = out_off[i + 1] - to;
+        warp_copy(seq + from, out_seq + to, len, lane);
+        if (qual) warp_copy(qual + from, out_qual + to, len, lane);
     }
 }
 

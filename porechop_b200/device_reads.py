@@ -1,0 +1,134 @@
+"""
+Porechop on reads that are already in GPU memory: trimmed and split output reads, with their qualities, in GPU memory.
+
+For callers whose reads live on the device (a basecaller on the same card, a torch pipeline): one
+adapterTrimSplitReadsDevice call runs Phase B (end trims), Phase C (middle adapters) and cuts the records Porechop writes --
+the records fastq.emit would write for the same decisions, in the same order -- into device tensors.  Only the decisions
+(trims, hits, barcode rankings) come to the host; the bases and qualities never do.
+
+    from porechop_b200 import device_reads, fastq
+    out = device_reads.trim_reads(seq, seq_off, matching_sets, (3, -6, -5, -2), qual)
+    # out.seq / out.qual / out.off / out.read / out.part: CUDA tensors; record r is seq[off[r]:off[r+1]] of read read[r],
+    # part[r] = 0 (not split) or k >= 1 (the k-th part).  To write files:
+    data = fastq.emit_parts(name_buf, name_off, rna, tuple(x.cpu().numpy() if x is not None else None
+                                                           for x in out[:5]), 'fastq')
+
+The device work runs on torch.cuda.current_stream(); the call returns when the outputs are written.  `W` (the engine's
+wrapper module) and `device()` (the allocator) are module attributes, so that the same set handling and retry logic can run
+on another engine build.
+"""
+import collections
+
+import numpy as np
+
+from . import cpp_function_wrappers as W
+from . import fastq
+
+TrimmedReads = collections.namedtuple('TrimmedReads', 'seq qual off read part start_trim end_trim hits calls')
+
+
+class TorchDevice:
+    """Device buffers as torch tensors on the current CUDA device; work on torch.cuda.current_stream()."""
+
+    def __init__(self):
+        import torch
+        self.torch = torch
+        self.dtypes = {np.uint8: torch.uint8, np.int32: torch.int32, np.int64: torch.int64}
+
+    def empty(self, n, dtype):
+        return self.torch.empty(int(n), dtype=self.dtypes[dtype], device='cuda')
+
+    def ptr(self, t):
+        return t.data_ptr() if t is not None else 0
+
+    def numel(self, t):
+        return t.numel()
+
+    def head(self, t, n):
+        return t[:int(n)]
+
+    def stream(self):
+        return self.torch.cuda.current_stream().cuda_stream
+
+    def check(self, seq, seq_off, qual):
+        torch = self.torch
+        for name, t, dt in (('seq', seq, torch.uint8), ('seq_off', seq_off, torch.int64), ('qual', qual, torch.uint8)):
+            if t is None:
+                continue
+            if not (t.is_cuda and t.dtype == dt and t.dim() == 1 and t.is_contiguous()):
+                raise ValueError('%s must be a contiguous 1-D %s CUDA tensor' % (name, dt))
+        if qual is not None and qual.numel() != seq.numel():
+            raise ValueError('qual must hold one quality per base, at the offsets of the reads')
+
+
+_device = None
+
+
+def device():
+    """the allocator trim_reads uses (a TorchDevice unless replaced)"""
+    global _device
+    if _device is None:
+        _device = TorchDevice()
+    return _device
+
+
+def initial_parts_cap(n):
+    """room for output records of the first attempt: every read plus a quarter split once (chimeras are a few per cent), then
+    one more call with the exact count when that is not enough"""
+    return n + n // 4 + 1024
+
+
+def trim_reads(seq, seq_off, matching_sets, scoring_scheme_vals, qual=None, *, end_size=150, extra_end_trim=2,
+               end_threshold=75.0, min_trim_size=4, no_split=False, middle_threshold=85.0, extra_middle_trim_good_side=10,
+               extra_middle_trim_bad_side=100, min_split_read_size=1000, discard_middle=False, untrimmed=False, barcodes=None):
+    """What `porechop` writes for reads in GPU memory, in GPU memory.  seq: uint8 bases, seq_off: int64[n + 1] offsets, qual:
+    uint8 qualities at the same offsets or None (FASTA); matching_sets and the options as for fastq.trim_fastq /
+    fastq.demux_fastq.  barcodes = dict(forward_or_reverse, barcode_threshold, barcode_diff, require_two_barcodes) also calls
+    the barcodes (determine_barcode) from the device's top-2 ranking.
+    Returns TrimmedReads: seq, qual (None without input qualities), off (int64[n_parts + 1]), read, part (int32[n_parts]) on
+    the device; start_trim / end_trim (host int32[n]), hits ({read: [(adapter position, start, end, score), ...]} as
+    fastq.find_middle_hits returns them) and calls (list of bin names, or None without barcodes)."""
+    D = device()
+    if hasattr(D, 'check'):
+        D.check(seq, seq_off, qual)
+    n = D.numel(seq_off) - 1
+    n_bytes = D.numel(seq)
+    sets = fastq._norm_sets(matching_sets)
+    starts = [s[1] for _, s, _ in sets if s]
+    ends = [e[1] for _, _, e in sets if e]
+    adapters = [] if no_split else fastq._middle_adapters(sets)
+    start_names, end_names = {s[0] for _, s, _ in sets if s}, {e[0] for _, _, e in sets if e}
+    # middle_trim_ranges: the bad side is before a start sequence's hit and after an end sequence's hit
+    left = [extra_middle_trim_bad_side if nm in start_names else extra_middle_trim_good_side for nm, _ in adapters]
+    right = [extra_middle_trim_bad_side if nm in end_names else extra_middle_trim_good_side for nm, _ in adapters]
+    s_cols, e_cols, su, eu = ([], [], [], []) if barcodes is None else \
+        fastq.barcode_columns(sets, barcodes.get('forward_or_reverse', 'forward'))
+    pk = lambda x: W.pack_sequences(x, offset_dtype=np.int32)     # noqa: E731
+    middle = pk([a[1] for a in adapters]) if adapters else None
+    cap = initial_parts_cap(n)
+    for attempt in range(2):
+        out_seq = D.empty(max(n_bytes, 1), np.uint8)
+        out_qual = D.empty(max(n_bytes, 1), np.uint8) if qual is not None else None
+        out_off, out_read, out_part = D.empty(cap + 1, np.int64), D.empty(max(cap, 1), np.int32), D.empty(max(cap, 1), np.int32)
+        try:
+            st, et, ss, es, n_hits, h, n_parts, n_out = W.adapter_trim_split_reads_device(
+                D.ptr(seq), D.ptr(seq_off), n, n_bytes, -1, pk(starts) + (s_cols,), pk(ends) + (e_cols,), middle,
+                scoring_scheme_vals, end_size, extra_end_trim, end_threshold, min_trim_size, middle_threshold,
+                want_top2=barcodes is not None, stream_ptr=D.stream(), d_quals_ptr=D.ptr(qual),
+                mid_extra=(left, right) if adapters else None, min_split_read_size=min_split_read_size,
+                discard_middle=discard_middle, untrimmed=untrimmed, d_out_seq_ptr=D.ptr(out_seq), d_out_qual_ptr=D.ptr(out_qual),
+                d_out_off_ptr=D.ptr(out_off), d_out_read_ptr=D.ptr(out_read), d_out_part_ptr=D.ptr(out_part), parts_cap=cap)
+        except W.EngineError as e:
+            if e.code == W.ERR_SPACE and attempt == 0 and getattr(e, 'n_parts', 0) > cap:
+                cap = e.n_parts                       # the exact number of records: one more call
+                continue
+            raise
+        break
+    calls = None
+    if barcodes is not None:
+        calls = fastq.call_barcodes_top2((su, fastq.Top2Scores(su, ss).ranked()), (eu, fastq.Top2Scores(eu, es).ranked()),
+                                         barcodes.get('barcode_threshold', 75.0), barcodes.get('barcode_diff', 5.0),
+                                         barcodes.get('require_two_barcodes', False))
+    return TrimmedReads(D.head(out_seq, n_out), D.head(out_qual, n_out) if out_qual is not None else None,
+                        D.head(out_off, n_parts + 1), D.head(out_read, n_parts), D.head(out_part, n_parts), st, et,
+                        fastq._hits_dict(n_hits, h), calls)

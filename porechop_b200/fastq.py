@@ -21,6 +21,7 @@ buffers end to end:
   middle_trim_ranges(...)    hits -> the ranges the reference adds to `middle_trim_positions`
   emit(...)                  get_fastq / get_fasta of every read (split parts, numbering, --discard_middle,
                              --min_split_read_size, RNA T->U) as one bytes object, assembled with vectorised scatters
+  emit_parts(...)            the same bytes for output records already cut on the device (device_reads.trim_reads)
   search_adapter_sets(...)   Phase A: best start / end identity of every adapter set over the check reads' windows --
                              or, with PB200_DEVICE_SEARCH=1, one adapterSetSearch call that reduces them on the device
   trim_fastq(...)            all of the above for a fixed list of adapter sets: what `porechop -i x.fastq -o y.fastq`
@@ -543,6 +544,51 @@ def emit(batch, start_trim=None, end_trim=None, middle=None, fmt='fastq', min_sp
     return np.frombuffer(out, dtype=np.uint8) if as_array else out
 
 
+def emit_parts(name_buf, name_off, rna, parts, fmt='fastq', select=None):
+    """The bytes Porechop writes for output records that were already cut (adapterTrimSplitReadsDevice, device_reads.trim_reads),
+    copied to the host: parts = (seq, qual, off, read, part) -- bases and qualities of record r at off[r] .. off[r + 1] (qual
+    None for FASTA), its source read and part number (0 = not split, k >= 1 = the k-th part, whose name gets '_k' the way
+    add_number_to_read_name does).  name_buf / name_off / rna: the source reads' names and RNA flags (FastqBatch fields); RNA
+    reads are written with U.  select (bool per source read) keeps the records of a subset, e.g. one barcode bin.  FASTA is
+    written in 70-column lines."""
+    seq, qual, off, read, part = parts
+    off = np.asarray(off, dtype=np.int64)
+    read = np.asarray(read, dtype=np.int64)
+    part = np.asarray(part, dtype=np.int64)
+    if fmt not in ('fastq', 'fasta'):
+        raise ValueError("fmt must be 'fastq' or 'fasta'")
+    if fmt == 'fastq' and qual is None:
+        raise ValueError('FASTQ output needs the qualities')
+    seq = np.ascontiguousarray(seq, dtype=np.uint8)
+    qual = seq if qual is None else np.ascontiguousarray(qual, dtype=np.uint8)
+    rec = np.arange(len(read)) if select is None else np.flatnonzero(np.asarray(select, dtype=bool)[read])
+    src = read[rec]
+    names, name_off = np.ascontiguousarray(name_buf, dtype=np.uint8), np.asarray(name_off, dtype=np.int64)
+    n0, nlen = name_off[src], name_off[src + 1] - name_off[src]
+    split = np.flatnonzero(part[rec] > 0)
+    if len(split):
+        nb = names.tobytes()
+        extra, extra_off = W.pack_sequences([_numbered_name(nb[n0[k]:n0[k] + nlen[k]], int(part[rec[k]])) for k in split],
+                                            offset_dtype=np.int64)
+        n0, nlen = n0.copy(), nlen.copy()
+        n0[split] = len(names) + extra_off[:-1]
+        nlen[split] = np.diff(extra_off)
+        names = np.concatenate([names, extra])
+    slen = off[rec + 1] - off[rec]
+    if fmt == 'fastq':
+        rec_len = 1 + nlen + 1 + slen + 3 + slen + 1
+    else:
+        rec_len = 1 + nlen + 1 + slen + (slen + 69) // 70
+    rna_rec = np.asarray(rna, dtype=bool)[read]                  # per record
+    if hostio.LIB is not None:
+        out_off = np.zeros(len(rec_len) + 1, dtype=np.int64)
+        np.cumsum(rec_len, out=out_off[1:])
+        return hostio.emit(out_off, fmt, names, n0, nlen, seq, off[rec], slen, qual, off[rec], slen, rna_rec[rec]).tobytes()
+    records = FastqBatch(names, None, seq, off, qual, off, rna_rec)   # one "read" per record
+    z = np.zeros(len(rec), dtype=np.int64)
+    return _assemble(records, names, fmt, rec, z, slen, z, slen, n0, nlen, rec_len) if len(rec) else b''
+
+
 def _assemble(batch, names, fmt, read, s0, slen, q0, qlen, n0, nlen, rec_len):
     off = np.zeros(len(rec_len) + 1, dtype=np.int64)
     np.cumsum(rec_len, out=off[1:])
@@ -724,6 +770,24 @@ def _dict_columns(names):
     return list(last.keys()), [last[nm] for nm in last]
 
 
+def barcode_columns(sets, forward_or_reverse):
+    """The barcode score columns of normalised adapter sets (_norm_sets) for one direction: (start columns, end columns,
+    start names, end names).  A set is a barcode if its name starts with 'Barcode ' (adapters.py:31-32); its direction is
+    'reverse' if its start name contains '_rev' (adapters.py:34-38).  Columns index the start / end adapters in set order;
+    the reference's score dicts hold every barcode name once (first position, last value), so exactly those columns are
+    ranked and each name is listed once."""
+    def is_bc(name, s):
+        return name.startswith('Barcode ') and (('reverse' if '_rev' in s[0] else 'forward') == forward_or_reverse)
+    s_sets = [t for t in sets if t[1]]
+    e_sets = [t for t in sets if t[2]]
+    s_cols = [j for j, (name, s, e) in enumerate(s_sets) if is_bc(name, s)]
+    e_cols = [j for j, (name, s, e) in enumerate(e_sets) if is_bc(name, s)]
+    s_names = [_barcode_name(*s_sets[j]) for j in s_cols]
+    e_names = [_barcode_name(*e_sets[j]) for j in e_cols]
+    (su, sk), (eu, ek) = _dict_columns(s_names), _dict_columns(e_names)
+    return [s_cols[k] for k in sk], [e_cols[k] for k in ek], su, eu
+
+
 def call_barcodes(start_scores, start_names, end_scores, end_names, barcode_threshold=75.0, barcode_diff=5.0,
                   require_two_barcodes=False, albacore_calls=None):
     """determine_barcode (nanopore_read.py:399-470) for all reads at once.  start_scores: float[n, len(start_names)]
@@ -849,18 +913,7 @@ def demux_fastq(data, matching_sets, scoring_scheme_vals, forward_or_reverse='fo
     (porechop.py:54-79, 652-676) once Phase A has chosen `matching_sets` = [(set name, start, end), ...] and the
     barcode direction.  A set is a barcode if its name starts with 'Barcode ' (adapters.py:31-32); its direction is
     'reverse' if its start name contains '_rev' (adapters.py:34-38).  Returns (bins, info)."""
-    def is_bc(name, s):
-        return name.startswith('Barcode ') and (('reverse' if '_rev' in s[0] else 'forward') == forward_or_reverse)
-    sets = _norm_sets(matching_sets)
-    s_sets = [t for t in sets if t[1]]
-    e_sets = [t for t in sets if t[2]]
-    s_cols = [j for j, (name, s, e) in enumerate(s_sets) if is_bc(name, s)]
-    e_cols = [j for j, (name, s, e) in enumerate(e_sets) if is_bc(name, s)]
-    s_names = [_barcode_name(*s_sets[j]) for j in s_cols]
-    e_names = [_barcode_name(*e_sets[j]) for j in e_cols]
-    # the reference's score dicts hold every barcode name once (first position, last value): rank exactly those columns
-    (su, sk), (eu, ek) = _dict_columns(s_names), _dict_columns(e_names)
-    s_cols, e_cols = [s_cols[k] for k in sk], [e_cols[k] for k in ek]
+    s_cols, e_cols, su, eu = barcode_columns(_norm_sets(matching_sets), forward_or_reverse)
     batch, sets, st, et, srec, erec, middle, seconds = _run_trim(data, matching_sets, scoring_scheme_vals, end_size,
                                                                  extra_end_trim, end_threshold, min_trim_size, no_split,
                                                                  middle_threshold, extra_middle_trim_good_side,

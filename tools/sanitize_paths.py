@@ -107,5 +107,26 @@ for end_size in (150, 200):
         return flat(got), flat((st, et, sp, ep, n_hits, h))
     run('trim', {}, trim)
     run('trim_dev', {}, lambda: trim(True))
+
+
+# output reads cut on the device (adapterTrimSplitReadsDevice): against fastq.emit over adapterTrimReads' decisions
+def split_reads():
+    import torch
+    from porechop_b200 import device_reads
+    qual = np.full(len(lbuf), ord('5'), dtype=np.uint8)
+    names, name_off = W.pack_sequences(['r%d' % k for k in range(len(loff) - 1)])
+    rna = np.zeros(len(loff) - 1, dtype=bool)
+    sets = [(('t', yt), ('b', yb))]
+    r = device_reads.trim_reads(torch.from_numpy(lbuf).cuda(), torch.from_numpy(loff).cuda(), sets, wl.DEFAULT_SCORING,
+                                torch.from_numpy(qual).cuda(), min_split_read_size=100)
+    got = fastq.emit_parts(names, name_off, rna, tuple(x.cpu().numpy() for x in r[:5]), 'fastq')
+    st, et, _, _, n_hits, h = W.adapter_trim_reads(lbuf, loff, sides[0], sides[1], (a2, o2), wl.DEFAULT_SCORING, 150, 2, 75.0, 4, 85.0)
+    middle = fastq.middle_trim_ranges(fastq._hits_dict(n_hits, h), [('t', yt), ('b', yb)], {'t'}, {'b'}, 10, 100)
+    batch = fastq.FastqBatch(names, name_off, lbuf, loff, qual, loff, rna)
+    exp = fastq.emit(batch, st, et, middle, 'fastq', 100)
+    return np.frombuffer(got, dtype=np.uint8), np.frombuffer(exp, dtype=np.uint8)
+
+
+run('split_dev', {}, split_reads)
 print('SANITIZE RUN COMPLETE, %d wrong' % bad, flush=True)
 sys.exit(1 if bad else 0)
