@@ -242,6 +242,41 @@ typedef struct {
 int adapterTrimSplitReadsDevice(const uint8_t *d_seqs, const int64_t *d_seq_off, int64_t n_seqs, int64_t total_seq_bytes,
                                 int64_t max_seq_len, const pb200_trim_args_t *args, const pb200_split_args_t *split,
                                 int matchScore, int mismatchScore, int gapOpenScore, int gapExtensionScore, void *stream);
+/* Porechop's demultiplexed output reads on the device (porechop -b DIR): adapterTrimSplitReadsDevice (same semantics, stream
+ * and ordering rules, status word, trims, hits and PB200_ERR_SPACE behaviour), plus the barcode call of every read, with the
+ * records grouped by bin.
+ *   - The call of a read is determine_barcode (porechop/nanopore_read.py:399-470) on the top-2 ranking of each side's score
+ *     columns (adapterEndDecisions' `top2`): the column's bin is start_bin[pos] / end_bin[pos], its score the exact double the
+ *     reference parses, float("%f" % (100.0 * match / len)), 0.0 when the side has no column.  Without require_two_barcodes
+ *     the best of both sides wins (the start side on ties) if it reaches barcode_threshold and beats by barcode_diff the best
+ *     entry of either side with another bin; with it both sides' best must agree, reach the threshold and beat their own
+ *     side's second by barcode_diff.  d_albacore[s] >= 0: the call stands only if it equals d_albacore[s] (Porechop and
+ *     Albacore must agree), else the read goes to 'none'.  read_bin[s] = the call (n_bins = 'none').
+ *   - Records are grouped by bin in bin-id order, 'none' last; inside a bin in read order, the parts of a read in position
+ *     order (the sequence fastq.demux_fastq writes into each bin's file).  bin_parts[b] .. bin_parts[b + 1] are the records
+ *     of bin b (b = n_bins: 'none'), their bases d_out_off[bin_parts[b]] .. d_out_off[bin_parts[b + 1]].
+ *   - discard_unassigned: the 'none' records are not written and do not count in *n_parts, *n_out_bases or parts_cap.
+ * On PB200_ERR_SPACE read_bin, bin_parts, the trims and the hits are valid; the device outputs are not.  The top2 outputs of
+ * args->start / args->end may be NULL (the ranking stays on the device).
+ * Preconditions, checked before the device is touched (PB200_ERR_ARG otherwise): those of adapterTrimSplitReadsDevice, demux /
+ * read_bin / bin_parts not NULL, start_bin / end_bin present when the side has score columns, bin ids in [0, n_bins) and no
+ * bin twice on one side, 0 <= n_bins < 4096, barcode_threshold / barcode_diff not NaN, and the side windows within the
+ * device ranking's domain (end_size + longest adapter + 2 <= 4095).  With no barcode columns every read is 'none'. */
+typedef struct {
+    const int32_t *start_bin;          /* host, args->start.n_score_cols: bin id of each start score column            */
+    const int32_t *end_bin;            /* host, args->end.n_score_cols: bin id of each end score column                */
+    int32_t n_bins;                    /* named bins 0 .. n_bins - 1; bin n_bins is 'none'                              */
+    double barcode_threshold, barcode_diff;
+    int32_t require_two_barcodes, discard_unassigned;
+    const int32_t *d_albacore;         /* device, per read, or NULL: -1 = no Albacore call, else the bin the call must
+                                          equal (n_bins + 1 = a name that is no bin: the read always goes to 'none')    */
+    int32_t *read_bin;                 /* host out, n_seqs: the call of every read (n_bins = 'none')                    */
+    int64_t *bin_parts;                /* host out, n_bins + 2: record offsets of the bins in output order              */
+} pb200_demux_args_t;
+int adapterDemuxReadsDevice(const uint8_t *d_seqs, const int64_t *d_seq_off, int64_t n_seqs, int64_t total_seq_bytes,
+                            int64_t max_seq_len, const pb200_trim_args_t *args, const pb200_split_args_t *split,
+                            const pb200_demux_args_t *demux, int matchScore, int mismatchScore, int gapOpenScore,
+                            int gapExtensionScore, void *stream);
 /* cmin[l], l = 0 .. len-1: the smallest c with float("%f" % (100.0*c/l)) >= middle_threshold, or l+1 if none does
  * (cmin[0] = INT32_MAX).  The ">=" sibling of pb200TrimThresholdTable.  Pure host code; middle_threshold must be > 0. */
 int pb200MiddleThresholdTable(double middle_threshold, int32_t len, int32_t *cmin);

@@ -111,6 +111,18 @@ class SplitArgsDesc(Structure):
 C_LIB.adapterTrimSplitReadsDevice.argtypes = [c_void_p, c_void_p, c_int64, c_int64, c_int64, POINTER(TrimArgsDesc),
                                               POINTER(SplitArgsDesc), c_int, c_int, c_int, c_int, c_void_p]
 C_LIB.adapterTrimSplitReadsDevice.restype = c_int
+
+
+class DemuxArgsDesc(Structure):
+    """pb200_demux_args_t (include/porechop_b200.h)"""
+    _fields_ = [('start_bin', c_void_p), ('end_bin', c_void_p), ('n_bins', c_int32), ('barcode_threshold', c_double),
+                ('barcode_diff', c_double), ('require_two_barcodes', c_int32), ('discard_unassigned', c_int32),
+                ('d_albacore', c_void_p), ('read_bin', c_void_p), ('bin_parts', c_void_p)]
+
+
+C_LIB.adapterDemuxReadsDevice.argtypes = [c_void_p, c_void_p, c_int64, c_int64, c_int64, POINTER(TrimArgsDesc),
+                                          POINTER(SplitArgsDesc), POINTER(DemuxArgsDesc), c_int, c_int, c_int, c_int, c_void_p]
+C_LIB.adapterDemuxReadsDevice.restype = c_int
 C_LIB.pb200MiddleThresholdTable.argtypes = [c_double, c_int32, c_void_p]
 C_LIB.pb200MiddleThresholdTable.restype = c_int
 C_LIB.pb200FormatRecord.argtypes = [c_void_p, c_char_p, c_int]
@@ -136,7 +148,7 @@ EXPORTED_SYMBOLS = ['adapterAlignment', 'freeCString', 'adapterAlignmentBatch', 
                     'adapterAlignmentBatchDevice', 'adapterEndDecisions', 'pb200TrimThresholdTable', 'adapterSetSearch',
                     'adapterMiddleScan',
                     'adapterMiddleScanDevice', 'pb200MiddleThresholdTable', 'adapterTrimReads', 'adapterTrimReadsDevice',
-                    'adapterTrimSplitReadsDevice', 'pb200FormatRecord', 'pb200DeviceCount', 'pb200SetDevice', 'pb200Synchronize', 'pb200LastError',
+                    'adapterTrimSplitReadsDevice', 'adapterDemuxReadsDevice', 'pb200FormatRecord', 'pb200DeviceCount', 'pb200SetDevice', 'pb200Synchronize', 'pb200LastError',
                     'pb200KernelLaunches', 'pb200TimingEnable', 'pb200TimingRead', 'pb200TimingReadKinds', 'pb200SetOption',
                     'pb200GetOption', 'pb200HostBuffer', 'pb200PackNibbles']
 
@@ -394,9 +406,10 @@ def adapter_middle_scan_device(d_seqs_ptr, d_seq_off_ptr, n_seqs, total_seq_byte
 
 
 def _trim_reads(call, n_seqs, start, end, middle, end_size, extra_trim_size, end_threshold, min_trim_size, middle_threshold,
-                want_top2):
+                want_top2, want_scores=True):
     """adapterTrimReads(Device) with caller-owned outputs: builds pb200_trim_args_t, starts with room for 2n + 1024 hits and
-    retries once with exactly *n_total when the engine answers PB200_ERR_SPACE (as _middle_scan)."""
+    retries once with exactly *n_total when the engine answers PB200_ERR_SPACE (as _middle_scan).  want_scores=False: no
+    score output at all (the demux stage ranks the columns on the device); the scores are then returned as None."""
     keep, sides, outs = [], [], []
     for ad_buf, ad_off, cols in (start, end):
         ad_buf = np.ascontiguousarray(ad_buf, dtype=np.uint8)
@@ -409,9 +422,10 @@ def _trim_reads(call, n_seqs, start, end, middle, end_size, extra_trim_size, end
             scores = np.zeros((n_seqs, len(cols), 2), dtype=np.uint16)
         keep.append((ad_buf, ad_off, cols))
         outs.append((trim, scores))
+        give = len(cols) and want_scores
         sides.append(TrimSideDesc(ad_buf.ctypes.data, ad_off.ctypes.data, len(ad_off) - 1, cols.ctypes.data if len(cols) else None,
-                                  len(cols), trim.ctypes.data, scores.ctypes.data if (len(cols) and not want_top2) else None,
-                                  scores.ctypes.data if (len(cols) and want_top2) else None))
+                                  len(cols), trim.ctypes.data, scores.ctypes.data if (give and not want_top2) else None,
+                                  scores.ctypes.data if (give and want_top2) else None))
     if middle is not None:
         mid_buf = np.ascontiguousarray(middle[0], dtype=np.uint8)
         mid_off = np.ascontiguousarray(middle[1], dtype=np.int32)
@@ -432,6 +446,8 @@ def _trim_reads(call, n_seqs, start, end, middle, end_size, extra_trim_size, end
         break
     _check(rc)
     (st, ss), (et, es) = outs
+    if not want_scores:
+        ss = es = None
     return st, et, ss, es, n_hits, hits[:total.value]
 
 
@@ -500,6 +516,48 @@ def adapter_trim_split_reads_device(d_seqs_ptr, d_seq_off_ptr, n_seqs, total_seq
         e.n_parts, e.n_out_bases = n_parts.value, n_bases.value
         raise
     return out + (n_parts.value, n_bases.value)
+
+
+def adapter_demux_reads_device(d_seqs_ptr, d_seq_off_ptr, n_seqs, total_seq_bytes, max_seq_len, start, end, middle,
+                               scoring_scheme_vals, end_size, extra_trim_size, end_threshold, min_trim_size, middle_threshold=85.0,
+                               stream_ptr=0, *, start_bin, end_bin, n_bins, barcode_threshold=75.0, barcode_diff=5.0,
+                               require_two_barcodes=False, discard_unassigned=False, d_albacore_ptr=0, d_quals_ptr=0,
+                               mid_extra=None, min_split_read_size=1000, discard_middle=False, untrimmed=False, d_out_seq_ptr=0,
+                               d_out_qual_ptr=0, d_out_off_ptr=0, d_out_read_ptr=0, d_out_part_ptr=0, parts_cap=0):
+    """adapter_trim_split_reads_device plus the barcode call of every read, with the records grouped by bin
+    (adapterDemuxReadsDevice).  start_bin / end_bin: the bin id of each start / end score column (start[2] / end[2]), bins
+    0 .. n_bins - 1 named, n_bins = 'none'; d_albacore_ptr: int32 per read on the device (-1 = no Albacore call), or 0.
+    Returns (start_trim, end_trim, n_hits, hits, n_parts, n_out_bases, read_bin int32[n], bin_parts int64[n_bins + 2]): the
+    records of bin b are bin_parts[b] .. bin_parts[b + 1].  When the kept records do not fit parts_cap it raises EngineError
+    with code ERR_SPACE and the totals as .n_parts / .n_out_bases (read_bin / bin_parts as .read_bin / .bin_parts)."""
+    ma, mi, go, ge = [int(x) for x in scoring_scheme_vals]
+    n_mid = len(middle[1]) - 1 if middle is not None else 0
+    left, right = mid_extra if mid_extra is not None else ([], [])
+    left = np.ascontiguousarray(left, dtype=np.int32)
+    right = np.ascontiguousarray(right, dtype=np.int32)
+    if len(left) != n_mid or len(right) != n_mid:
+        raise ValueError('mid_extra needs one (left, right) value per middle adapter')
+    start_bin = np.ascontiguousarray(start_bin, dtype=np.int32)
+    end_bin = np.ascontiguousarray(end_bin, dtype=np.int32)
+    read_bin = np.zeros(int(n_seqs), dtype=np.int32)
+    bin_parts = np.zeros(int(n_bins) + 2, dtype=np.int64)
+    n_parts, n_bases = c_int64(0), c_int64(0)
+    split = SplitArgsDesc(d_quals_ptr or None, left.ctypes.data if n_mid else None, right.ctypes.data if n_mid else None,
+                          int(min_split_read_size), int(bool(discard_middle)), int(bool(untrimmed)), d_out_seq_ptr or None,
+                          d_out_qual_ptr or None, d_out_off_ptr or None, d_out_read_ptr or None, d_out_part_ptr or None,
+                          int(parts_cap), addressof(n_parts), addressof(n_bases))
+    demux = DemuxArgsDesc(start_bin.ctypes.data if len(start_bin) else None, end_bin.ctypes.data if len(end_bin) else None,
+                          int(n_bins), float(barcode_threshold), float(barcode_diff), int(bool(require_two_barcodes)),
+                          int(bool(discard_unassigned)), d_albacore_ptr or None, read_bin.ctypes.data, bin_parts.ctypes.data)
+    try:
+        st, et, _, _, n_hits, hits = _trim_reads(lambda args: C_LIB.adapterDemuxReadsDevice(
+            c_void_p(d_seqs_ptr), c_void_p(d_seq_off_ptr), n_seqs, total_seq_bytes, max_seq_len, args, byref(split), byref(demux),
+            ma, mi, go, ge, c_void_p(stream_ptr)), int(n_seqs), start, end, middle, end_size, extra_trim_size, end_threshold,
+            min_trim_size, middle_threshold, False, want_scores=False)
+    except EngineError as e:
+        e.n_parts, e.n_out_bases, e.read_bin, e.bin_parts = n_parts.value, n_bases.value, read_bin, bin_parts
+        raise
+    return st, et, n_hits, hits, n_parts.value, n_bases.value, read_bin, bin_parts
 
 
 def middle_threshold_table(middle_threshold, length):

@@ -721,4 +721,41 @@ PB_HD int64_t split_runs(int64_t len, const int32_t *rng, int32_t n_rng, int64_t
     return k;
 }
 
+// Barcode call of the demux stage (adapterDemuxReadsDevice): determine_barcode (nanopore_read.py:399-470) from the two best
+// score columns of each side -- bin ids b1 / b2 (-1 = no such column) and their scores s1 / s2 (the exact doubles the
+// reference parses; 0.0 for no column).  A bin occurs at most once per side, so the best and second-best of the merged,
+// stably sorted list are among these four.  Only additions and comparisons: no contraction can change a result.
+// Returns the bin, n_bins = 'none'.
+struct BarcodeSide { int32_t b1, b2; double s1, s2; };
+PB_HD int32_t barcode_call(const BarcodeSide &s, const BarcodeSide &e, int32_t n_bins, double threshold, double diff,
+                           int32_t require_two, int32_t albacore) {
+    const int32_t none = n_bins;
+    int32_t call = none;
+    if (require_two) {
+        const int32_t sb = s.b1 >= 0 ? s.b1 : none, eb = e.b1 >= 0 ? e.b1 : none;
+        if (s.s1 >= threshold && e.s1 >= threshold && s.s1 >= s.s2 + diff && e.s1 >= e.s2 + diff && sb == eb) call = sb;
+    } else {
+        const bool have_s = s.b1 >= 0, have_e = e.b1 >= 0;
+        const bool s_first = have_s && (!have_e || s.s1 >= e.s1);     // the start list comes first on ties (stable sort)
+        const int32_t best_id = s_first ? s.b1 : have_e ? e.b1 : none;
+        const double best = s_first ? s.s1 : have_e ? e.s1 : 0.0;
+        // the best entry of each side with another bin than the winner's (its first or its second); 0.0 if there is none
+        bool any = false;
+        double second = 0.0;
+        const BarcodeSide *sides[2] = {&s, &e};
+        for (int k = 0; k < 2; ++k) {
+            const BarcodeSide &x = *sides[k];
+            const bool first = x.b1 >= 0 && x.b1 != best_id, other = !first && x.b2 >= 0 && x.b2 != best_id;
+            if (first || other) {
+                const double v = first ? x.s1 : x.s2;
+                if (!any || v > second) second = v;
+                any = true;
+            }
+        }
+        if (best >= threshold && best >= second + diff) call = best_id;
+    }
+    if (albacore >= 0 && albacore != call) call = none;          // Porechop and Albacore must agree
+    return call;
+}
+
 }  // namespace pb

@@ -197,6 +197,11 @@ struct Engine {
     // output stage (adapterTrimSplitReadsDevice): the segment's hit reads, their CSR of extended hit ranges, hit row per read,
     // records and bases per read (scanned in place), source offset per record
     DevBuf split_hits, split_rng_off, split_rng, split_hit_of, split_cnt, split_bytes, split_src;
+    // demux stage (adapterDemuxReadsDevice): the segment's top-2 rankings per side, bin of each score column per side, score
+    // table, the call-wide bin per read; the call's records in read order (source offset, offsets, read, part), the (key x
+    // tile) counts, bin offsets, kept bases, and the permuted source offsets
+    DevBuf demux_top2[2], demux_map[2], demux_tab, demux_bin, demux_rsrc, demux_roff, demux_rread, demux_rpart, demux_cnt,
+        demux_parts, demux_kept, demux_perm;
     // adapter-set search (adapterSetSearch): NSTAGE slices of search_cols u64 keys, one per stage, so that stages running at
     // once never share an accumulator; a batch owns the columns [search_col, search_col + n_adapters) of every slice
     DevBuf search_acc;
@@ -972,9 +977,11 @@ struct Packer {
 
 // decide_kernel over the records of `cnt` reads (the reads s0 .. s0+cnt-1 of decision batch D) on `stream`: the trims go to
 // d_trim (the stage's chunk scratch, or a segment-wide array that later kernels read) and are copied home with the score
-// pairs / top2 of the chunk into D's host outputs.
+// pairs / top2 of the chunk into D's host outputs.  d_top2: the top2 ranking goes there instead (a device array that later
+// kernels read), and home only when D.top2 is given.
 int launch_decide(Engine &E, Stage &S, cudaStream_t stream, const pb200_end_batch_t &D, const int32_t *records, int64_t cnt,
-                  int32_t n_adapters, const int32_t *d_cmin, int32_t cmin_len, const int32_t *d_cols, int32_t *d_trim, int64_t s0) {
+                  int32_t n_adapters, const int32_t *d_cmin, int32_t cmin_len, const int32_t *d_cols, int32_t *d_trim, int64_t s0,
+                  int32_t *d_top2 = nullptr) {
     if (int rc = S.dec_pairs.ensure((size_t)cnt * std::max<int32_t>(D.n_score_cols, 1) * 4)) return rc;
     DecideArgs a;
     a.records = records; a.n = cnt; a.n_adapters = n_adapters;
@@ -983,7 +990,9 @@ int launch_decide(Engine &E, Stage &S, cudaStream_t stream, const pb200_end_batc
     a.trim = d_trim;
     a.pairs = (D.score_pairs && D.n_score_cols > 0) ? S.dec_pairs.as<uint32_t>() : nullptr;
     a.top2 = nullptr;
-    if (D.top2) {
+    if (d_top2) {
+        a.top2 = d_top2;
+    } else if (D.top2) {
         if (int rc = S.dec_top2.ensure((size_t)cnt * 6 * 4)) return rc;
         a.top2 = S.dec_top2.as<int32_t>();
     }
@@ -995,8 +1004,8 @@ int launch_decide(Engine &E, Stage &S, cudaStream_t stream, const pb200_end_batc
     if (a.pairs)
         CK(cudaMemcpyAsync(D.score_pairs + (size_t)s0 * D.n_score_cols * 2, S.dec_pairs.p,
                            (size_t)cnt * D.n_score_cols * 4, cudaMemcpyDeviceToHost, stream));
-    if (a.top2)
-        CK(cudaMemcpyAsync(D.top2 + (size_t)s0 * 6, S.dec_top2.p, (size_t)cnt * 6 * 4, cudaMemcpyDeviceToHost, stream));
+    if (a.top2 && D.top2)
+        CK(cudaMemcpyAsync(D.top2 + (size_t)s0 * 6, a.top2, (size_t)cnt * 6 * 4, cudaMemcpyDeviceToHost, stream));
     return 0;
 }
 
@@ -1867,11 +1876,12 @@ int scan_offsets(Engine &E, cudaStream_t stream, int64_t *x, int64_t n) {
 }
 
 // One side of Phase B: preconditions (those of adapterEndDecisions plus int16 classes with a finite window bound) and the
-// threshold table's length.
-int trim_side_check(const pb200_trim_side_t &T, int64_t n_seqs, int32_t end_size, const SchemeInfo &si, int32_t *cmin_len) {
+// threshold table's length.  rank: the demux stage ranks the score columns on the device (top2 may then be NULL).
+int trim_side_check(const pb200_trim_side_t &T, int64_t n_seqs, int32_t end_size, const SchemeInfo &si, int32_t *cmin_len,
+                    bool rank = false) {
     if (T.n_adapters < 0 || T.n_score_cols < 0) return fail(PB200_ERR_ARG, "negative count");
     if (n_seqs > 0 && !T.trim) return fail(PB200_ERR_ARG, "NULL pointer");
-    if (T.n_score_cols > 0 && ((!T.score_pairs && !T.top2) || !T.score_cols)) return fail(PB200_ERR_ARG, "NULL pointer");
+    if (T.n_score_cols > 0 && ((!T.score_pairs && !T.top2 && !rank) || !T.score_cols)) return fail(PB200_ERR_ARG, "NULL pointer");
     for (int32_t k = 0; k < T.n_score_cols; ++k)
         if (T.score_cols[k] < 0 || T.score_cols[k] >= T.n_adapters) return fail(PB200_ERR_ARG, "score column out of range");
     *cmin_len = 0;
@@ -1886,7 +1896,7 @@ int trim_side_check(const pb200_trim_side_t &T, int64_t n_seqs, int32_t end_size
         m_max = std::max<int64_t>(m_max, m);
     }
     if ((int64_t)end_size + m_max + 2 > 65535) return fail(PB200_ERR_ARG, "windows too long for the device decisions");
-    if (T.top2 && ((int64_t)end_size + m_max + 2 > 4095 || T.n_score_cols >= 0xFFFF))
+    if ((T.top2 || (rank && T.n_score_cols > 0)) && ((int64_t)end_size + m_max + 2 > 4095 || T.n_score_cols >= 0xFFFF))
         return fail(PB200_ERR_ARG, "windows too long / too many score columns for the device barcode ranking");
     *cmin_len = (int32_t)(end_size + m_max + 2);
     return 0;
@@ -1895,13 +1905,16 @@ int trim_side_check(const pb200_trim_side_t &T, int64_t n_seqs, int32_t end_size
 // The reads [a, b) of the next segment: the middle scan's budget (middle_segment_end) with, per read, the two end windows (and
 // their codes when they are encoded), window offsets, two trims, the trimmed range's first base and -- host API -- the
 // segment's ASCII reads and offsets next to their codes.
-// split: the output stage's buffers too (hit row, records and bases per read, the source offset of up to two records per read).
+// split: the output stage's buffers too (hit row, records and bases per read, the source offset of up to two records per read);
+// demux: the two sides' top-2 rankings.
 int64_t trim_segment_end(const Engine &E, int64_t a, int64_t n_seqs, int32_t n_mid, int64_t wl_max, const int64_t *h_seq_off,
-                         bool split = false) {
+                         bool split = false, bool demux = false) {
     size_t held = E.trim_reads.cap + E.trim_off.cap + E.trim_win_off.cap + E.trim_win[0].cap + E.trim_win[1].cap +
                   E.trim_d[0].cap + E.trim_d[1].cap + E.trim_first.cap;
     if (split) held += E.split_hit_of.cap + E.split_cnt.cap + E.split_bytes.cap + E.split_src.cap;
-    int64_t b = middle_segment_end(E, a, n_seqs, n_mid, h_seq_off, 3.0 * (double)wl_max + 40 + (split ? 44.0 : 0.0),
+    if (demux) held += E.demux_top2[0].cap + E.demux_top2[1].cap;
+    int64_t b = middle_segment_end(E, a, n_seqs, n_mid, h_seq_off,
+                                   3.0 * (double)wl_max + 40 + (split ? 44.0 : 0.0) + (demux ? 48.0 : 0.0),
                                    h_seq_off ? 2.0 : 1.0, held);
 #ifdef PB_TEST_SEGMENT_READS
     // tests of the host-simulated engine only (through sim_engine.load): small segments, so that a few reads span several
@@ -1914,11 +1927,50 @@ int64_t trim_segment_end(const Engine &E, int64_t a, int64_t n_seqs, int32_t n_m
 // (once they do not, the stage only counts).
 struct SplitTotals { int64_t parts = 0, bases = 0; bool write = true; };
 
+// Demux stage of adapterDemuxReadsDevice: the shape of the score table (tab_c match counts x tab_l lengths; 0 x 0 without
+// barcode columns).
+struct DemuxStage {
+    int32_t tab_c = 0, tab_l = 0;
+};
+
+// tab[c * l_n + l] = percent_exact(c, max(l, 1)) for c < c_n, l < l_n: the barcode scores of the top-2 pairs (match_ad, len_ad),
+// the doubles Top2Scores.ranked() gives them.  A pure function of the shape: built once, reused by every later call.
+std::shared_ptr<const std::vector<double>> cached_score_table(int32_t c_n, int32_t l_n) {
+    static std::mutex mu;
+    static std::map<std::pair<int32_t, int32_t>, std::shared_ptr<const std::vector<double>>> cache;
+    std::lock_guard<std::mutex> lk(mu);
+    const auto key = std::make_pair(c_n, l_n);
+    auto it = cache.find(key);
+    if (it != cache.end()) return it->second;
+    auto t = std::make_shared<std::vector<double>>((size_t)c_n * (size_t)l_n);
+    for (int32_t c = 0; c < c_n; ++c)
+        for (int32_t l = 0; l < l_n; ++l) (*t)[(size_t)c * l_n + l] = percent_exact(c, std::max<int32_t>(l, 1));
+    if (cache.size() >= 16) cache.clear();                     // growth guard (window shapes are few in practice)
+    cache[key] = t;
+    return t;
+}
+
+// b grown to at least `bytes` with its first `keep` bytes kept (copied on `stream`): the call-wide record arrays of the demux
+// stage, which grow segment by segment
+int grow_keep(DevBuf &b, size_t bytes, size_t keep, cudaStream_t stream) {
+    if (bytes <= b.cap) return 0;
+    DevBuf g;
+    if (int rc = g.ensure(bytes)) return rc;
+    if (keep) CK(cudaMemcpyAsync(g.p, b.p, keep, cudaMemcpyDeviceToDevice, stream));
+    CK(cudaStreamSynchronize(stream));
+    if (b.p) cudaFree(b.p);
+    b.p = g.p;
+    b.cap = g.cap;
+    return 0;
+}
+
 // One segment's records [a, a + n): reads at reads[off[s] ..], trimmed ranges first[s] / toff (scanned lengths) on the device;
 // the segment's hits are the rounds from rounds[r0] on (segment-relative reads, {adapter, record} each).
+// Dm: the records go to the demux stage's call-wide arrays in read order (their bins group them once all are known), not to
+// the caller's buffers.
 int split_segment(Engine &E, cudaStream_t stream, const pb200_split_args_t &X, const uint8_t *reads, const int64_t *off, int64_t a,
                   int64_t n, const int64_t *first, const int64_t *toff, const std::vector<MiddleRound> &rounds, size_t r0,
-                  SplitTotals &T) {
+                  SplitTotals &T, const DemuxStage *Dm = nullptr) {
     // ---- the hit reads and their extended ranges (rs - left, re + right) sorted by start: a CSR, a few ints per hit ----
     struct Rng { int32_t read, x, y; };
     std::vector<Rng> all;
@@ -1976,18 +2028,33 @@ int split_segment(Engine &E, cudaStream_t stream, const pb200_split_args_t &X, c
     CK(cudaMemcpyAsync(&seg[0], cnt + n, 8, cudaMemcpyDeviceToHost, stream));
     CK(cudaMemcpyAsync(&seg[1], bytes + n, 8, cudaMemcpyDeviceToHost, stream));
     CK(cudaStreamSynchronize(stream));
-    if (T.write && T.parts + seg[0] > X.parts_cap) T.write = false;     // PB200_ERR_SPACE: from here on only count
-    if (T.write) {
-        // ---- each record's output offset, read, part and source; then the gather, one warp per record ----
-        if (int rc = E.split_src.ensure((size_t)seg[0] * 8 + 16)) return rc;
-        int64_t *src = E.split_src.as<int64_t>();
+    if (!Dm && T.write && T.parts + seg[0] > X.parts_cap) T.write = false;     // PB200_ERR_SPACE: from here on only count
+    if (Dm || T.write) {
+        // ---- each record's output offset, read, part and source; then the gather, one warp per record.  Demux: the records
+        // are appended to the call's records in read order instead, and gathered once their bins are known ----
+        int64_t *src, *rec_off = X.d_out_off;
+        int32_t *rec_read = X.d_out_read, *rec_part = X.d_out_part;
+        if (Dm) {
+            const size_t n_rec = (size_t)(T.parts + seg[0]), have = (size_t)T.parts;
+            if (int rc = grow_keep(E.demux_rsrc, n_rec * 8 + 16, have * 8, stream)) return rc;
+            if (int rc = grow_keep(E.demux_roff, (n_rec + 1) * 8 + 16, have * 8, stream)) return rc;
+            if (int rc = grow_keep(E.demux_rread, n_rec * 4 + 16, have * 4, stream)) return rc;
+            if (int rc = grow_keep(E.demux_rpart, n_rec * 4 + 16, have * 4, stream)) return rc;
+            src = E.demux_rsrc.as<int64_t>() + T.parts;
+            rec_off = E.demux_roff.as<int64_t>();
+            rec_read = E.demux_rread.as<int32_t>();
+            rec_part = E.demux_rpart.as<int32_t>();
+        } else {
+            if (int rc = E.split_src.ensure((size_t)seg[0] * 8 + 16)) return rc;
+            src = E.split_src.as<int64_t>();
+        }
         split_write_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(off, first, toff, hit_of, rng_off_d, rng_d, n, min_split,
                                                                             X.discard_middle, X.untrimmed,
                                                                             static_cast<const int64_t *>(cnt),
                                                                             static_cast<const int64_t *>(bytes), T.parts, T.bases, a,
-                                                                            src, X.d_out_off, X.d_out_read, X.d_out_part);
+                                                                            src, rec_off, rec_read, rec_part);
         g_launches++;
-        if (seg[0] > 0) {
+        if (!Dm && seg[0] > 0) {
             const int64_t blocks = std::max<int64_t>(1, std::min<int64_t>((seg[0] + 7) / 8, (int64_t)E.sm_count * 8));
             split_gather_kernel<<<(unsigned)blocks, 256, 0, stream>>>(reads, X.d_quals, static_cast<const int64_t *>(src),
                                                                       static_cast<const int64_t *>(X.d_out_off + T.parts), seg[0],
@@ -2001,11 +2068,76 @@ int split_segment(Engine &E, cudaStream_t stream, const pb200_split_args_t &X, c
     return 0;
 }
 
+// Demux stage, once per call after the last segment: the read bins come home, the call's records (T.parts of them, in read
+// order) are partitioned stably by bin into the caller's buffers, and the bin offsets come home.  T becomes the totals of the
+// records that are kept; when they do not fit parts_cap nothing is written (the caller reports PB200_ERR_SPACE).
+int demux_finalize(Engine &E, Stage &S, cudaStream_t stream, const pb200_split_args_t &X, const pb200_demux_args_t &Dm,
+                   const uint8_t *seqs, int64_t n_seqs, SplitTotals &T) {
+    const int64_t n_rec = T.parts;
+    const int32_t n_bins = Dm.n_bins, n_keys = n_bins + 2;              // the bins, 'none', dropped
+    const int64_t tiles = (n_rec + PB_DEMUX_TILE - 1) / PB_DEMUX_TILE;
+    const int32_t *read_bin = E.demux_bin.as<int32_t>();
+    CK(cudaMemcpyAsync(Dm.read_bin, read_bin, (size_t)n_seqs * 4, cudaMemcpyDeviceToHost, stream));
+    std::vector<int64_t> parts((size_t)n_keys + 1, 0);
+    unsigned long long kept_bytes = 0;
+    int64_t *cnt = nullptr;
+    if (n_rec > 0) {
+        // ---- (key x tile) counts, scanned key-major: every (key, tile) its first output record; the key offsets come home ----
+        const int64_t m = (int64_t)n_keys * tiles;
+        if (int rc = E.demux_cnt.ensure((size_t)(m + 1) * 8)) return rc;
+        if (int rc = E.demux_parts.ensure((size_t)(n_keys + 1) * 8)) return rc;
+        if (int rc = E.demux_kept.ensure(16)) return rc;
+        cnt = E.demux_cnt.as<int64_t>();
+        CK(cudaMemsetAsync(E.demux_kept.p, 0, 8, stream));
+        demux_count_kernel<<<(unsigned)tiles, PB_DEMUX_TILE, 0, stream>>>(static_cast<const int32_t *>(E.demux_rread.as<int32_t>()),
+                                                                          static_cast<const int64_t *>(E.demux_roff.as<int64_t>()), n_rec,
+                                                                          read_bin, n_bins, Dm.discard_unassigned, tiles,
+                                                                          cnt, E.demux_kept.as<unsigned long long>());
+        g_launches++;
+        CK(cudaGetLastError());
+        if (int rc = scan_offsets(E, stream, cnt, m)) return rc;
+        demux_bin_parts_kernel<<<(unsigned)((n_keys + 1 + 255) / 256), 256, 0, stream>>>(static_cast<const int64_t *>(cnt), tiles,
+                                                                                          n_keys, E.demux_parts.as<int64_t>());
+        g_launches++;
+        CK(cudaGetLastError());
+        CK(cudaMemcpyAsync(parts.data(), E.demux_parts.p, (size_t)(n_keys + 1) * 8, cudaMemcpyDeviceToHost, stream));
+        CK(cudaMemcpyAsync(&kept_bytes, E.demux_kept.p, 8, cudaMemcpyDeviceToHost, stream));
+    }
+    if (int rc = check_status(S, stream)) return rc;    // (synchronises the stream) a score outside the table
+    memcpy(Dm.bin_parts, parts.data(), (size_t)(n_bins + 2) * 8);
+    const int64_t kept = parts[(size_t)n_bins + 1];
+    T.parts = kept;
+    T.bases = (int64_t)kept_bytes;
+    if (kept > X.parts_cap) return 0;
+    // ---- the kept records in bin order: lengths (scanned into offsets), reads, parts, permuted sources; then the gather ----
+    CK(cudaMemsetAsync(X.d_out_off, 0, 8, stream));
+    if (kept > 0) {
+        if (int rc = E.demux_perm.ensure((size_t)kept * 8 + 16)) return rc;
+        int64_t *perm = E.demux_perm.as<int64_t>();
+        demux_scatter_kernel<<<(unsigned)tiles, PB_DEMUX_TILE, 0, stream>>>(
+            static_cast<const int32_t *>(E.demux_rread.as<int32_t>()), static_cast<const int32_t *>(E.demux_rpart.as<int32_t>()),
+            static_cast<const int64_t *>(E.demux_roff.as<int64_t>()), static_cast<const int64_t *>(E.demux_rsrc.as<int64_t>()), n_rec,
+            read_bin, n_bins, Dm.discard_unassigned, tiles, static_cast<const int64_t *>(cnt), X.d_out_off + 1, X.d_out_read,
+            X.d_out_part, perm);
+        g_launches++;
+        CK(cudaGetLastError());
+        if (int rc = scan_offsets(E, stream, X.d_out_off, kept)) return rc;
+        const int64_t blocks = std::max<int64_t>(1, std::min<int64_t>((kept + 7) / 8, (int64_t)E.sm_count * 8));
+        split_gather_kernel<<<(unsigned)blocks, 256, 0, stream>>>(seqs, X.d_quals, static_cast<const int64_t *>(perm),
+                                                                  static_cast<const int64_t *>(X.d_out_off), kept, X.d_out_seq,
+                                                                  X.d_out_qual);
+        g_launches++;
+        CK(cudaGetLastError());
+    }
+    return 0;
+}
+
 // device: seqs / seq_off are device pointers (adapterTrimReadsDevice), else host buffers uploaded segment by segment.
-// X: the output stage of adapterTrimSplitReadsDevice (device reads only), or nullptr.
+// X: the output stage of adapterTrimSplitReadsDevice (device reads only), or nullptr.  Dm: the demux stage of
+// adapterDemuxReadsDevice (with X), or nullptr.
 int trim_reads(const uint8_t *seqs, const int64_t *seq_off, int64_t n_seqs, bool device, int64_t total_seq_bytes,
                int64_t max_seq_len, const pb200_trim_args_t *A, int ma, int mi, int go, int ge, void *user_stream,
-               const pb200_split_args_t *X = nullptr) {
+               const pb200_split_args_t *X = nullptr, const pb200_demux_args_t *Dm = nullptr) {
     // ---- preconditions: nothing below touches the device before they all hold ----
     if (!A) return fail(PB200_ERR_ARG, "NULL pointer");
     if (n_seqs < 0 || total_seq_bytes < 0) return fail(PB200_ERR_ARG, "negative count");
@@ -2016,7 +2148,7 @@ int trim_reads(const uint8_t *seqs, const int64_t *seq_off, int64_t n_seqs, bool
     const pb200_trim_side_t *side[2] = {&A->start, &A->end};
     int32_t cmin_len[2] = {0, 0}, mid_cmin_len = 0;
     for (int k = 0; k < 2; ++k)
-        if (int rc = trim_side_check(*side[k], n_seqs, A->end_size, si, &cmin_len[k])) return rc;
+        if (int rc = trim_side_check(*side[k], n_seqs, A->end_size, si, &cmin_len[k], Dm != nullptr)) return rc;
     const int32_t n_mid = A->n_mid_adapters;
     if (n_mid < 0) return fail(PB200_ERR_ARG, "negative count");
     if (n_mid > 0) {
@@ -2048,6 +2180,31 @@ int trim_reads(const uint8_t *seqs, const int64_t *seq_off, int64_t n_seqs, bool
                                                                   (total_seq_bytes > 0 && !X->d_out_seq)))))
             return fail(PB200_ERR_ARG, "NULL pointer");
     }
+    DemuxStage dstage;
+    if (Dm) {
+        if (!X) return fail(PB200_ERR_ARG, "the demux stage needs the output stage");
+        if (!Dm->read_bin || !Dm->bin_parts) return fail(PB200_ERR_ARG, "NULL pointer");
+        if (Dm->n_bins < 0 || Dm->n_bins >= 4096) return fail(PB200_ERR_ARG, "n_bins must be in [0, 4096)");
+        if (std::isnan(Dm->barcode_threshold) || std::isnan(Dm->barcode_diff))
+            return fail(PB200_ERR_ARG, "barcode_threshold / barcode_diff is NaN");
+        std::vector<char> seen((size_t)Dm->n_bins);
+        for (int k = 0; k < 2; ++k) {
+            const int32_t *map = k ? Dm->end_bin : Dm->start_bin;
+            const int32_t n_cols = side[k]->n_score_cols;
+            if (n_cols == 0) continue;
+            if (!map) return fail(PB200_ERR_ARG, "NULL pointer");
+            std::fill(seen.begin(), seen.end(), 0);
+            for (int32_t j = 0; j < n_cols; ++j) {
+                if (map[j] < 0 || map[j] >= Dm->n_bins) return fail(PB200_ERR_ARG, "bin id out of range");
+                if (seen[(size_t)map[j]]) return fail(PB200_ERR_ARG, "a bin appears twice on one side");
+                seen[(size_t)map[j]] = 1;
+            }
+            // the score table covers every (match_ad, len_ad) of the side: match_ad <= its longest adapter, len_ad < cmin_len
+            dstage.tab_c = std::max(dstage.tab_c, cmin_len[k] - A->end_size - 1);
+            dstage.tab_l = std::max(dstage.tab_l, cmin_len[k]);
+        }
+        memset(Dm->bin_parts, 0, (size_t)(Dm->n_bins + 2) * 8);
+    }
     if (A->n_hits && n_seqs > 0) memset(A->n_hits, 0, (size_t)n_seqs * 4);
     if (A->n_total) *A->n_total = 0;
     for (int k = 0; k < 2; ++k) {         // a side without adapters: nothing aligns, nothing is trimmed
@@ -2068,7 +2225,7 @@ int trim_reads(const uint8_t *seqs, const int64_t *seq_off, int64_t n_seqs, bool
     cudaStream_t stream = S.stream;
     if (device) { if (int rc = library_stream(E, user_stream, &stream)) return rc; }
     if (int rc = order_after_last(E, stream)) return rc;
-    NvtxRange submit_range(X ? "pb200:submit_trim_split" : "pb200:submit_trim");
+    NvtxRange submit_range(Dm ? "pb200:submit_demux" : X ? "pb200:submit_trim_split" : "pb200:submit_trim");
     std::vector<MiddleRound> rounds;
     SplitTotals totals;
     auto run = [&]() -> int {
@@ -2086,6 +2243,21 @@ int trim_reads(const uint8_t *seqs, const int64_t *seq_off, int64_t n_seqs, bool
             if (T.n_score_cols > 0)
                 CK(cudaMemcpyAsync(E.dec_cols[k].p, T.score_cols, (size_t)T.n_score_cols * 4, cudaMemcpyHostToDevice, stream));
         }
+        if (Dm) {                             // the call rule's inputs: bin of each score column, score table; a bin per read
+            for (int k = 0; k < 2; ++k) {
+                const int32_t n_cols = side[k]->n_score_cols;
+                if (n_cols == 0) continue;
+                if (int rc = E.demux_map[k].ensure((size_t)n_cols * 4)) return rc;
+                CK(cudaMemcpyAsync(E.demux_map[k].p, k ? Dm->end_bin : Dm->start_bin, (size_t)n_cols * 4, cudaMemcpyHostToDevice,
+                                   stream));
+            }
+            if (dstage.tab_c > 0) {
+                const auto tab = cached_score_table(dstage.tab_c, dstage.tab_l);
+                if (int rc = E.demux_tab.ensure(tab->size() * 8)) return rc;
+                CK(cudaMemcpyAsync(E.demux_tab.p, tab->data(), tab->size() * 8, cudaMemcpyHostToDevice, stream));
+            }
+            if (int rc = E.demux_bin.ensure((size_t)n_seqs * 4 + 16)) return rc;
+        }
         if (n_mid > 0) {
             if (int rc = plan_adapters(E, stream, A->mid_adapters, A->mid_ad_off, n_mid, ma, mi, go, ge, PM)) return rc;
             if (int rc = middle_table(E, stream, A->middle_threshold, mid_cmin_len)) return rc;   // (synchronises the stream)
@@ -2099,7 +2271,7 @@ int trim_reads(const uint8_t *seqs, const int64_t *seq_off, int64_t n_seqs, bool
             if (int rc = E.mid_codes.ensure((size_t)total_seq_bytes + 16)) return rc;
         }
         for (int64_t a = 0; a < n_seqs;) {
-            const int64_t b = trim_segment_end(E, a, n_seqs, n_mid, wl_max, device ? nullptr : seq_off, X != nullptr);
+            const int64_t b = trim_segment_end(E, a, n_seqs, n_mid, wl_max, device ? nullptr : seq_off, X != nullptr, Dm != nullptr);
             const int64_t n = b - a;
             // the segment's reads: ASCII at reads[off[s] .. off[s+1])
             const uint8_t *reads = seqs;
@@ -2157,15 +2329,32 @@ int trim_reads(const uint8_t *seqs, const int64_t *seq_off, int64_t n_seqs, bool
                 D.score_cols = T.score_cols; D.n_score_cols = T.n_score_cols;
                 D.trim = T.trim; D.score_pairs = T.score_pairs; D.top2 = T.top2;
                 const int64_t max_cnt = std::max<int64_t>(1, g_opt.device_chunk_tasks / T.n_adapters);
+                int32_t *top2 = nullptr;     // demux: the segment's ranking stays on the device for barcode_call_kernel
+                if (Dm && T.n_score_cols > 0) {
+                    if (int rc = E.demux_top2[k].ensure((size_t)n * 6 * 4 + 16)) return rc;
+                    top2 = E.demux_top2[k].as<int32_t>();
+                }
                 for (int64_t c0 = 0; c0 < n; c0 += max_cnt) {
                     const int64_t cnt = std::min(max_cnt, n - c0);
                     if (int rc = S.out.ensure((size_t)cnt * T.n_adapters * PB_REC * 4)) return rc;
                     if (int rc = run_cross_chunk(E, S, stream, P[k], w, win_off + c0, cnt, 0, wl_max, T.n_adapters,
                                                  S.out.as<int32_t>(), nullptr, 0, T.ad_off, nullptr, ascii)) return rc;
                     if (int rc = launch_decide(E, S, stream, D, S.out.as<int32_t>(), cnt, T.n_adapters, E.dec_cmin[k].as<int32_t>(),
-                                               cmin_len[k], E.dec_cols[k].as<int32_t>(), E.trim_d[k].as<int32_t>() + c0, a + c0))
+                                               cmin_len[k], E.dec_cols[k].as<int32_t>(), E.trim_d[k].as<int32_t>() + c0, a + c0,
+                                               top2 ? top2 + c0 * 6 : nullptr))
                         return rc;
                 }
+            }
+            if (Dm) {                        // ---- the barcode call of every read of the segment ----
+                const int32_t *t[2] = {nullptr, nullptr};
+                for (int k = 0; k < 2; ++k) if (side[k]->n_score_cols > 0) t[k] = E.demux_top2[k].as<int32_t>();
+                barcode_call_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(
+                    t[0], t[1], static_cast<const int32_t *>(E.demux_map[0].as<int32_t>()),
+                    static_cast<const int32_t *>(E.demux_map[1].as<int32_t>()), static_cast<const double *>(E.demux_tab.as<double>()),
+                    dstage.tab_c, dstage.tab_l, n, Dm->n_bins, Dm->barcode_threshold, Dm->barcode_diff, Dm->require_two_barcodes,
+                    Dm->d_albacore ? Dm->d_albacore + a : nullptr, E.demux_bin.as<int32_t>() + a, S.misc.as<int>());
+                g_launches++;
+                CK(cudaGetLastError());
             }
             if (n_mid == 0) {
                 if (int rc = check_status(S, stream)) return rc;
@@ -2179,7 +2368,7 @@ int trim_reads(const uint8_t *seqs, const int64_t *seq_off, int64_t n_seqs, bool
                     g_launches++;
                     if (int rc = scan_offsets(E, stream, toff, n)) return rc;
                     if (int rc = split_segment(E, stream, *X, reads, off, a, n, E.trim_first.as<int64_t>(), toff, rounds, rounds.size(),
-                                               totals)) return rc;
+                                               totals, Dm ? &dstage : nullptr)) return rc;
                 }
                 a = b;
                 continue;
@@ -2213,10 +2402,14 @@ int trim_reads(const uint8_t *seqs, const int64_t *seq_off, int64_t n_seqs, bool
             const size_t r0 = rounds.size();
             if (int rc = middle_rounds(E, S, stream, PM, M, n_mid, A->mid_ad_off, a, rounds)) return rc;
             if (X) {
-                if (int rc = split_segment(E, stream, *X, reads, off, a, n, E.trim_first.as<int64_t>(), M.off, rounds, r0, totals))
+                if (int rc = split_segment(E, stream, *X, reads, off, a, n, E.trim_first.as<int64_t>(), M.off, rounds, r0, totals,
+                                           Dm ? &dstage : nullptr))
                     return rc;
             }
             a = b;
+        }
+        if (Dm) {
+            if (int rc = demux_finalize(E, S, stream, *X, *Dm, seqs, n_seqs, totals)) return rc;
         }
         if (X) CK(cudaStreamSynchronize(stream));      // the device outputs are written when the call returns
         return 0;
@@ -2307,6 +2500,17 @@ int adapterTrimSplitReadsDevice(const uint8_t *d_seqs, const int64_t *d_seq_off,
     if (split->n_parts) *split->n_parts = 0;
     if (split->n_out_bases) *split->n_out_bases = 0;
     return trim_reads(d_seqs, d_seq_off, n_seqs, true, total_seq_bytes, max_seq_len, args, ma, mi, go, ge, stream, split);
+}
+
+int adapterDemuxReadsDevice(const uint8_t *d_seqs, const int64_t *d_seq_off, int64_t n_seqs, int64_t total_seq_bytes,
+                            int64_t max_seq_len, const pb200_trim_args_t *args, const pb200_split_args_t *split,
+                            const pb200_demux_args_t *demux, int ma, int mi, int go, int ge, void *stream) {
+    g_err.clear();
+    if (!split) return fail(PB200_ERR_ARG, "NULL pointer");
+    if (split->n_parts) *split->n_parts = 0;
+    if (split->n_out_bases) *split->n_out_bases = 0;
+    if (!demux) return fail(PB200_ERR_ARG, "NULL pointer");
+    return trim_reads(d_seqs, d_seq_off, n_seqs, true, total_seq_bytes, max_seq_len, args, ma, mi, go, ge, stream, split, demux);
 }
 
 int pb200MiddleThresholdTable(double middle_threshold, int32_t len, int32_t *cmin) {

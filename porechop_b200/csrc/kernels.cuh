@@ -13,6 +13,8 @@
 //                        cut from resident reads, trims turned into the trimmed reads the middle scan masks
 //   split_mark / split_count / split_write / split_gather: output stage of adapterTrimSplitReadsDevice -- Porechop's output
 //                        records counted, placed and gathered (bases + qualities) into the caller's buffers
+//   barcode_call / demux_count / demux_bin_parts / demux_scatter: demux stage of adapterDemuxReadsDevice -- the barcode call
+//                        of every read, and the records partitioned stably by bin before split_gather copies them
 //   generic_kernel       int32 thread-serial fallback for scoring schemes / adapters outside the int16 domain
 //
 // The arithmetic is in dp_core.cuh (shared with the CPU emulation used by the tests).
@@ -1265,6 +1267,117 @@ __global__ void __launch_bounds__(256) split_gather_kernel(const uint8_t *__rest
         warp_copy(seq + from, out_seq + to, len, lane);
         if (qual) warp_copy(qual + from, out_qual + to, len, lane);
     }
+}
+
+// ---------------------------------------------------------------------------------------------------
+// Demux stage of adapterDemuxReadsDevice.  Per segment, barcode_call_kernel turns the two sides' top-2 rankings (decide_kernel)
+// into each read's bin.  Once per call, after the last segment, the records the output stage placed in read order (engine
+// scratch: source offset, offsets, read, part) are partitioned stably by key = their read's bin ('none' = n_bins, or
+// n_bins + 1 = dropped with discard_unassigned): a histogram per tile of PB_DEMUX_TILE records, the scan of the (key x tile)
+// counts in key-major order, then a scatter that keeps the read order inside each tile.  split_gather_kernel then copies the
+// bases from the permuted source offsets.
+#define PB_DEMUX_TILE 256
+#define PB_DEMUX_MAX_KEYS 4097                 // n_bins < 4096: the named bins, 'none', dropped
+
+// read_bin[s] of the segment's reads: top2_* = decide_kernel's 6 ints per read of a side (NULL: the side has no barcode
+// column), bin_* = bin of each score column, tab[c * tab_l + l] = float("%f" % (100.0 * c / max(l, 1))) for c < tab_c,
+// l < tab_l; albacore = the reads' Albacore bins or NULL.  A pair outside the table sets status bit 2.
+__device__ __forceinline__ BarcodeSide barcode_side(const int32_t *t, const int32_t *bin, const double *tab, int32_t tab_c,
+                                                     int32_t tab_l, int *status) {
+    BarcodeSide x = {-1, -1, 0.0, 0.0};
+    if (!t) return x;
+    for (int k = 0; k < 2; ++k) {
+        const int32_t pos = t[3 * k], c = t[3 * k + 1], l = t[3 * k + 2];
+        if (pos < 0) continue;
+        double v = 0.0;
+        if (c < 0 || c >= tab_c || l < 0 || l >= tab_l) atomicOr(status, 2);
+        else v = tab[(int64_t)c * tab_l + l];
+        if (k == 0) { x.b1 = bin[pos]; x.s1 = v; } else { x.b2 = bin[pos]; x.s2 = v; }
+    }
+    return x;
+}
+__global__ void barcode_call_kernel(const int32_t *top2_s, const int32_t *top2_e, const int32_t *bin_s, const int32_t *bin_e,
+                                    const double *tab, int32_t tab_c, int32_t tab_l, int64_t n, int32_t n_bins, double threshold,
+                                    double diff, int32_t require_two, const int32_t *albacore, int32_t *read_bin, int *status) {
+    const int64_t s = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (s >= n) return;
+    const BarcodeSide bs = barcode_side(top2_s ? top2_s + s * 6 : nullptr, bin_s, tab, tab_c, tab_l, status);
+    const BarcodeSide be = barcode_side(top2_e ? top2_e + s * 6 : nullptr, bin_e, tab, tab_c, tab_l, status);
+    read_bin[s] = barcode_call(bs, be, n_bins, threshold, diff, require_two, albacore ? albacore[s] : -1);
+}
+// the partition key of record r (-1 past the last record)
+__device__ __forceinline__ int32_t demux_key(const int32_t *rec_read, const int32_t *read_bin, int64_t r, int64_t n_rec,
+                                             int32_t n_bins, int32_t discard) {
+    if (r >= n_rec) return -1;
+    const int32_t b = read_bin[rec_read[r]];
+    return (discard && b == n_bins) ? n_bins + 1 : b;
+}
+// counts of the keys in tile t -> cnt[1 + k * tiles + t] (cnt[0] = 0, for scan_offsets); the bases of the records that are
+// kept (key <= n_bins) are added to *kept_bytes.  One block of PB_DEMUX_TILE threads per tile.
+__global__ void __launch_bounds__(PB_DEMUX_TILE) demux_count_kernel(const int32_t *rec_read, const int64_t *rec_off, int64_t n_rec,
+                                                                    const int32_t *read_bin, int32_t n_bins, int32_t discard,
+                                                                    int64_t tiles, int64_t *cnt, unsigned long long *kept_bytes) {
+    __shared__ unsigned hist[PB_DEMUX_MAX_KEYS];
+    __shared__ unsigned long long bytes;
+    const int32_t n_keys = n_bins + 2;
+    for (int32_t k = threadIdx.x; k < n_keys; k += blockDim.x) hist[k] = 0u;
+    if (threadIdx.x == 0) bytes = 0ull;
+    if (blockIdx.x == 0 && threadIdx.x == 0) cnt[0] = 0;
+    __syncthreads();
+    const int64_t r = (int64_t)blockIdx.x * PB_DEMUX_TILE + threadIdx.x;
+    const int32_t key = demux_key(rec_read, read_bin, r, n_rec, n_bins, discard);
+    if (key >= 0) {
+        atomicAdd(&hist[key], 1u);
+        if (key <= n_bins) atomicAdd(&bytes, (unsigned long long)(rec_off[r + 1] - rec_off[r]));
+    }
+    __syncthreads();
+    for (int32_t k = threadIdx.x; k < n_keys; k += blockDim.x) cnt[1 + (int64_t)k * tiles + blockIdx.x] = hist[k];
+    if (threadIdx.x == 0 && bytes) atomicAdd(kept_bytes, bytes);
+}
+// parts[k] = base[k * tiles], k = 0 .. n_keys: the first record of every key in output order, then the total
+__global__ void demux_bin_parts_kernel(const int64_t *base, int64_t tiles, int32_t n_keys, int64_t *parts) {
+    const int32_t k = (int32_t)(blockIdx.x * blockDim.x + threadIdx.x);
+    if (k <= n_keys) parts[k] = base[(int64_t)k * tiles];
+}
+// Stable scatter: record r of tile t with key k goes to base[k * tiles + t] + (the records of key k before it in the tile).
+// Within a warp that rank comes from the keys of the lower lanes (shuffles); across the warps of the block a running count
+// per key in shared memory, updated one warp after the other.  Kept records write their length to out_len (d_out_off + 1,
+// scanned afterwards), read, part and source offset; dropped ones (key n_bins + 1) write nothing.
+__global__ void __launch_bounds__(PB_DEMUX_TILE) demux_scatter_kernel(const int32_t *rec_read, const int32_t *rec_part,
+                                                                      const int64_t *rec_off, const int64_t *rec_src,
+                                                                      int64_t n_rec, const int32_t *read_bin, int32_t n_bins,
+                                                                      int32_t discard, int64_t tiles, const int64_t *base,
+                                                                      int64_t *out_len, int32_t *out_read, int32_t *out_part,
+                                                                      int64_t *perm_src) {
+    __shared__ unsigned run[PB_DEMUX_MAX_KEYS];
+    const int32_t n_keys = n_bins + 2;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, n_warps = blockDim.x >> 5;
+    for (int32_t k = threadIdx.x; k < n_keys; k += blockDim.x) run[k] = 0u;
+    const int64_t r = (int64_t)blockIdx.x * PB_DEMUX_TILE + threadIdx.x;
+    const int32_t key = demux_key(rec_read, read_bin, r, n_rec, n_bins, discard);
+    unsigned before = 0;                        // lanes below with the same key
+    bool last = true;                           // no lane above with the same key
+    for (int j = 0; j < 32; ++j) {
+        const int32_t kj = __shfl_sync(0xffffffffu, key, j);
+        if (kj == key) {
+            if (j < lane) ++before;
+            if (j > lane) last = false;
+        }
+    }
+    __syncthreads();
+    unsigned rank = 0;
+    for (int w = 0; w < n_warps; ++w) {
+        if (warp == w && key >= 0) rank = run[key] + before;
+        __syncthreads();
+        if (warp == w && key >= 0 && last) run[key] = rank + 1;
+        __syncthreads();
+    }
+    if (key < 0 || key > n_bins) return;
+    const int64_t d = base[(int64_t)key * tiles + blockIdx.x] + rank;
+    out_len[d] = rec_off[r + 1] - rec_off[r];
+    out_read[d] = rec_read[r];
+    out_part[d] = rec_part[r];
+    perm_src[d] = rec_src[r];
 }
 
 // ---------------------------------------------------------------------------------------------------

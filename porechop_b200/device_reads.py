@@ -13,6 +13,16 @@ the records fastq.emit would write for the same decisions, in the same order -- 
     data = fastq.emit_parts(name_buf, name_off, rna, tuple(x.cpu().numpy() if x is not None else None
                                                            for x in out[:5]), 'fastq')
 
+demux_reads does the same for `porechop -b DIR`: it also calls every read's barcode on the device and returns the records
+grouped by bin, so that each bin's reads are one contiguous slice of records and bytes:
+
+    out = device_reads.demux_reads(seq, seq_off, matching_sets, (3, -6, -5, -2), qual, forward_or_reverse='forward',
+                                   barcode_threshold=75.0, barcode_diff=5.0, require_two_barcodes=False,
+                                   discard_unassigned=False)
+    for name, (r0, r1) in out.bins.items():          # the bytes demux_fastq writes into <name>.fastq
+        parts = (out.seq, out.qual, out.off[r0:r1 + 1], out.read[r0:r1], out.part[r0:r1])
+        data = fastq.emit_parts(name_buf, name_off, rna, tuple(x.cpu().numpy() for x in parts), 'fastq')
+
 The device work runs on torch.cuda.current_stream(); the call returns when the outputs are written.  `W` (the engine's
 wrapper module) and `device()` (the allocator) are module attributes, so that the same set handling and retry logic can run
 on another engine build.
@@ -25,6 +35,7 @@ from . import cpp_function_wrappers as W
 from . import fastq
 
 TrimmedReads = collections.namedtuple('TrimmedReads', 'seq qual off read part start_trim end_trim hits calls')
+DemuxedReads = collections.namedtuple('DemuxedReads', 'seq qual off read part bins calls start_trim end_trim hits')
 
 
 class TorchDevice:
@@ -49,6 +60,9 @@ class TorchDevice:
 
     def stream(self):
         return self.torch.cuda.current_stream().cuda_stream
+
+    def upload(self, arr):
+        return self.torch.from_numpy(np.ascontiguousarray(arr)).to('cuda')
 
     def check(self, seq, seq_off, qual):
         torch = self.torch
@@ -93,14 +107,8 @@ def trim_reads(seq, seq_off, matching_sets, scoring_scheme_vals, qual=None, *, e
         D.check(seq, seq_off, qual)
     n = D.numel(seq_off) - 1
     n_bytes = D.numel(seq)
-    sets = fastq._norm_sets(matching_sets)
-    starts = [s[1] for _, s, _ in sets if s]
-    ends = [e[1] for _, _, e in sets if e]
-    adapters = [] if no_split else fastq._middle_adapters(sets)
-    start_names, end_names = {s[0] for _, s, _ in sets if s}, {e[0] for _, _, e in sets if e}
-    # middle_trim_ranges: the bad side is before a start sequence's hit and after an end sequence's hit
-    left = [extra_middle_trim_bad_side if nm in start_names else extra_middle_trim_good_side for nm, _ in adapters]
-    right = [extra_middle_trim_bad_side if nm in end_names else extra_middle_trim_good_side for nm, _ in adapters]
+    sets, starts, ends, adapters, left, right = _options(matching_sets, no_split, extra_middle_trim_good_side,
+                                                         extra_middle_trim_bad_side)
     s_cols, e_cols, su, eu = ([], [], [], []) if barcodes is None else \
         fastq.barcode_columns(sets, barcodes.get('forward_or_reverse', 'forward'))
     pk = lambda x: W.pack_sequences(x, offset_dtype=np.int32)     # noqa: E731
@@ -132,3 +140,73 @@ def trim_reads(seq, seq_off, matching_sets, scoring_scheme_vals, qual=None, *, e
     return TrimmedReads(D.head(out_seq, n_out), D.head(out_qual, n_out) if out_qual is not None else None,
                         D.head(out_off, n_parts + 1), D.head(out_read, n_parts), D.head(out_part, n_parts), st, et,
                         fastq._hits_dict(n_hits, h), calls)
+
+
+def _options(matching_sets, no_split, extra_middle_trim_good_side, extra_middle_trim_bad_side):
+    """normalised sets, start / end adapters, middle adapters and their extra trims (middle_trim_ranges: the bad side is
+    before a start sequence's hit and after an end sequence's hit)"""
+    sets = fastq._norm_sets(matching_sets)
+    starts = [s[1] for _, s, _ in sets if s]
+    ends = [e[1] for _, _, e in sets if e]
+    adapters = [] if no_split else fastq._middle_adapters(sets)
+    start_names, end_names = {s[0] for _, s, _ in sets if s}, {e[0] for _, _, e in sets if e}
+    left = [extra_middle_trim_bad_side if nm in start_names else extra_middle_trim_good_side for nm, _ in adapters]
+    right = [extra_middle_trim_bad_side if nm in end_names else extra_middle_trim_good_side for nm, _ in adapters]
+    return sets, starts, ends, adapters, left, right
+
+
+def demux_reads(seq, seq_off, matching_sets, scoring_scheme_vals, qual=None, *, forward_or_reverse, barcode_threshold,
+                barcode_diff, require_two_barcodes, discard_unassigned, albacore_calls=None, end_size=150, extra_end_trim=2,
+                end_threshold=75.0, min_trim_size=4, no_split=False, middle_threshold=85.0, extra_middle_trim_good_side=10,
+                extra_middle_trim_bad_side=100, min_split_read_size=1000, discard_middle=False, untrimmed=False):
+    """What `porechop -b DIR` writes for reads in GPU memory, in GPU memory and grouped by bin (one
+    adapterDemuxReadsDevice call).  Arguments as trim_reads, plus the barcode options of fastq.demux_fastq; albacore_calls:
+    one bin name (or None) per read, or None.
+    Returns DemuxedReads: seq, qual, off, read, part on the device as in trim_reads, with the records grouped by bin (bins in
+    the order of the barcode names, 'none' last; read order inside a bin); bins = {name: (first record, end record)} for the
+    bins that have records; calls (one bin name per read, demux_fastq's info['calls']); start_trim / end_trim / hits as
+    trim_reads returns them."""
+    D = device()
+    if hasattr(D, 'check'):
+        D.check(seq, seq_off, qual)
+    n = D.numel(seq_off) - 1
+    n_bytes = D.numel(seq)
+    sets, starts, ends, adapters, left, right = _options(matching_sets, no_split, extra_middle_trim_good_side,
+                                                         extra_middle_trim_bad_side)
+    s_cols, e_cols, su, eu = fastq.barcode_columns(sets, forward_or_reverse)
+    names = list(dict.fromkeys(su + eu))
+    idx = {nm: i for i, nm in enumerate(names)}
+    n_bins = len(names)
+    alb = None
+    if albacore_calls is not None:
+        if len(albacore_calls) != n:
+            raise ValueError('albacore_calls needs one entry per read')
+        alb = D.upload(np.array([-1 if a is None else idx.get(a, n_bins + 1) for a in albacore_calls], dtype=np.int32))
+    pk = lambda x: W.pack_sequences(x, offset_dtype=np.int32)     # noqa: E731
+    middle = pk([a[1] for a in adapters]) if adapters else None
+    cap = initial_parts_cap(n)
+    for attempt in range(2):
+        out_seq = D.empty(max(n_bytes, 1), np.uint8)
+        out_qual = D.empty(max(n_bytes, 1), np.uint8) if qual is not None else None
+        out_off, out_read, out_part = D.empty(cap + 1, np.int64), D.empty(max(cap, 1), np.int32), D.empty(max(cap, 1), np.int32)
+        try:
+            st, et, n_hits, h, n_parts, n_out, read_bin, bin_parts = W.adapter_demux_reads_device(
+                D.ptr(seq), D.ptr(seq_off), n, n_bytes, -1, pk(starts) + (s_cols,), pk(ends) + (e_cols,), middle,
+                scoring_scheme_vals, end_size, extra_end_trim, end_threshold, min_trim_size, middle_threshold,
+                stream_ptr=D.stream(), start_bin=[idx[nm] for nm in su], end_bin=[idx[nm] for nm in eu], n_bins=n_bins,
+                barcode_threshold=barcode_threshold, barcode_diff=barcode_diff, require_two_barcodes=require_two_barcodes,
+                discard_unassigned=discard_unassigned, d_albacore_ptr=D.ptr(alb), d_quals_ptr=D.ptr(qual),
+                mid_extra=(left, right) if adapters else None, min_split_read_size=min_split_read_size,
+                discard_middle=discard_middle, untrimmed=untrimmed, d_out_seq_ptr=D.ptr(out_seq), d_out_qual_ptr=D.ptr(out_qual),
+                d_out_off_ptr=D.ptr(out_off), d_out_read_ptr=D.ptr(out_read), d_out_part_ptr=D.ptr(out_part), parts_cap=cap)
+        except W.EngineError as e:
+            if e.code == W.ERR_SPACE and attempt == 0 and getattr(e, 'n_parts', 0) > cap:
+                cap = e.n_parts                       # the exact number of records: one more call
+                continue
+            raise
+        break
+    bin_names = names + ['none']
+    bins = {bin_names[b]: (int(bin_parts[b]), int(bin_parts[b + 1])) for b in range(n_bins + 1) if bin_parts[b + 1] > bin_parts[b]}
+    return DemuxedReads(D.head(out_seq, n_out), D.head(out_qual, n_out) if out_qual is not None else None,
+                        D.head(out_off, n_parts + 1), D.head(out_read, n_parts), D.head(out_part, n_parts), bins,
+                        [bin_names[b] for b in read_bin.tolist()], st, et, fastq._hits_dict(n_hits, h))

@@ -128,5 +128,32 @@ def split_reads():
 
 
 run('split_dev', {}, split_reads)
+
+
+# demultiplexed output reads (adapterDemuxReadsDevice): each bin's bytes against fastq.demux_fastq, over 12 barcode sets
+def demux_reads():
+    import torch
+    from porechop_b200 import device_reads
+    bs, be = wl.demux_adapters()
+    buf, off = wl.synth_reads(8, bs[3] + yt, yb + be[3], seed=3, chimera_p=0.5, max_len=4000)
+    qual = np.full(len(buf), ord('5'), dtype=np.uint8)
+    n = len(off) - 1
+    names, name_off = W.pack_sequences(['r%d' % k for k in range(n)])
+    batch = fastq.FastqBatch(names, name_off, buf, off, qual, off, np.zeros(n, dtype=bool))
+    sets = [('Y', ('t', yt), ('b', yb))] + [('Barcode %d (forward)' % (j + 1), ('BC%02d' % (j + 1), bs[j]),
+                                             ('BC%02d_end' % (j + 1), be[j])) for j in range(12)]
+    bc = dict(forward_or_reverse='forward', barcode_threshold=75.0, barcode_diff=5.0, require_two_barcodes=False,
+              discard_unassigned=False)
+    r = device_reads.demux_reads(torch.from_numpy(buf).cuda(), torch.from_numpy(off).cuda(), sets, wl.DEFAULT_SCORING,
+                                 torch.from_numpy(qual).cuda(), min_split_read_size=100, **bc)
+    parts = tuple(x.cpu().numpy() for x in r[:5])
+    got = b''.join(fastq.emit_parts(names, name_off, batch.rna, parts[:2] + (parts[2][r0:r1 + 1], parts[3][r0:r1],
+                                                                            parts[4][r0:r1]), 'fastq') for r0, r1 in r.bins.values())
+    bins, _ = fastq.demux_fastq(batch, sets, wl.DEFAULT_SCORING, min_split_read_size=100, **bc)
+    exp = b''.join(bins[k] for k in r.bins) if sorted(bins) == sorted(r.bins) else b''
+    return np.frombuffer(got, dtype=np.uint8), np.frombuffer(exp, dtype=np.uint8)
+
+
+run('demux_dev', {}, demux_reads)
 print('SANITIZE RUN COMPLETE, %d wrong' % bad, flush=True)
 sys.exit(1 if bad else 0)
