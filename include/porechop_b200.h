@@ -277,6 +277,40 @@ int adapterDemuxReadsDevice(const uint8_t *d_seqs, const int64_t *d_seq_off, int
                             int64_t max_seq_len, const pb200_trim_args_t *args, const pb200_split_args_t *split,
                             const pb200_demux_args_t *demux, int matchScore, int mismatchScore, int gapOpenScore,
                             int gapExtensionScore, void *stream);
+/* The bytes Porechop writes for output records already in device memory -- e.g. those of adapterTrimSplitReadsDevice or
+ * adapterDemuxReadsDevice, or any slice of them (one bin) -- into a caller-owned device buffer: the bytes fastq.emit_parts
+ * writes for the same records, in record order (get_fastq / get_fasta, porechop/nanopore_read.py:97-147).
+ *   - FASTQ: '@' name' '\n' bases' '\n' '+' '\n' quals '\n'.  FASTA: '>' name' '\n', then bases' in lines of 70, each ending in
+ *     '\n' (no base line for a record without bases).
+ *   - name' is the source read's name; for part k >= 1 the decimal tag "_k" goes before its first 0x20 byte, or at its end when
+ *     it has none (add_number_to_read_name, nanopore_read.py:494-498).
+ *   - bases' are the stored bytes, except that records of a read with d_rna[read] != 0 have every 'T' written as 'U' (and only
+ *     'T').  Qualities are written as stored.
+ * d_out_off gets every record's byte offset (0 for the first; the scanned lengths) and *n_out_bytes the total.  If the total
+ * exceeds out_cap the call returns PB200_ERR_SPACE: *n_out_bytes and d_out_off are valid, d_out is not written.  The call
+ * returns once the device outputs are written; stream and ordering rules as adapterTrimReadsDevice (NULL: the library's own
+ * stream after the legacy default stream; after the work earlier calls of this library left queued; a deferred error in the
+ * status word is reported).
+ * Preconditions, checked before the device is touched (PB200_ERR_ARG otherwise): args not NULL, fmt 0 or 1, d_qual for FASTQ,
+ * no negative count, and the pointers the sizes need (n_out_bytes and d_out_off always).  The record arrays are checked on the
+ * device before anything is written to d_out (PB200_ERR_ARG, d_out untouched): 0 <= d_off[r] <= d_off[r + 1] <= seq_bytes,
+ * 0 <= d_read[r] < n_reads, d_part[r] >= 0 and 0 <= d_name_off[read] <= d_name_off[read + 1] <= name_bytes. */
+typedef struct {
+    const uint8_t *d_seq, *d_qual;     /* device: record bases / qualities at the same offsets; d_qual NULL: FASTA only       */
+    int64_t seq_bytes;                 /* length of d_seq (and d_qual)                                                        */
+    const int64_t *d_off;              /* device, n_rec + 1: record r = d_seq[d_off[r] .. d_off[r + 1]) (absolute offsets)    */
+    const int32_t *d_read, *d_part;    /* device, n_rec: source read; 0 = not split, k >= 1 = the k-th part                   */
+    const uint8_t *d_names;            /* device: the source reads' names, read s at d_names[d_name_off[s] .. d_name_off[s+1]) */
+    const int64_t *d_name_off;         /* device, n_reads + 1                                                                 */
+    int64_t n_reads, name_bytes;
+    const uint8_t *d_rna;              /* device, n_reads, or NULL: nonzero = RNA read (T written as U)                       */
+    int32_t fmt;                       /* 0 = FASTQ, 1 = FASTA                                                                */
+    uint8_t *d_out;                    /* device, out_cap bytes                                                               */
+    int64_t out_cap;
+    int64_t *d_out_off;                /* device out, n_rec + 1: byte offset of every record, then the total                 */
+    int64_t *n_out_bytes;              /* host out, always written                                                            */
+} pb200_emit_args_t;
+int pb200EmitReadsDevice(const pb200_emit_args_t *args, int64_t n_rec, void *stream);
 /* cmin[l], l = 0 .. len-1: the smallest c with float("%f" % (100.0*c/l)) >= middle_threshold, or l+1 if none does
  * (cmin[0] = INT32_MAX).  The ">=" sibling of pb200TrimThresholdTable.  Pure host code; middle_threshold must be > 0. */
 int pb200MiddleThresholdTable(double middle_threshold, int32_t len, int32_t *cmin);

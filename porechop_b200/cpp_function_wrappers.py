@@ -123,6 +123,18 @@ class DemuxArgsDesc(Structure):
 C_LIB.adapterDemuxReadsDevice.argtypes = [c_void_p, c_void_p, c_int64, c_int64, c_int64, POINTER(TrimArgsDesc),
                                           POINTER(SplitArgsDesc), POINTER(DemuxArgsDesc), c_int, c_int, c_int, c_int, c_void_p]
 C_LIB.adapterDemuxReadsDevice.restype = c_int
+
+
+class EmitArgsDesc(Structure):
+    """pb200_emit_args_t (include/porechop_b200.h)"""
+    _fields_ = [('d_seq', c_void_p), ('d_qual', c_void_p), ('seq_bytes', c_int64), ('d_off', c_void_p), ('d_read', c_void_p),
+                ('d_part', c_void_p), ('d_names', c_void_p), ('d_name_off', c_void_p), ('n_reads', c_int64),
+                ('name_bytes', c_int64), ('d_rna', c_void_p), ('fmt', c_int32), ('d_out', c_void_p), ('out_cap', c_int64),
+                ('d_out_off', c_void_p), ('n_out_bytes', c_void_p)]
+
+
+C_LIB.pb200EmitReadsDevice.argtypes = [POINTER(EmitArgsDesc), c_int64, c_void_p]
+C_LIB.pb200EmitReadsDevice.restype = c_int
 C_LIB.pb200MiddleThresholdTable.argtypes = [c_double, c_int32, c_void_p]
 C_LIB.pb200MiddleThresholdTable.restype = c_int
 C_LIB.pb200FormatRecord.argtypes = [c_void_p, c_char_p, c_int]
@@ -148,7 +160,7 @@ EXPORTED_SYMBOLS = ['adapterAlignment', 'freeCString', 'adapterAlignmentBatch', 
                     'adapterAlignmentBatchDevice', 'adapterEndDecisions', 'pb200TrimThresholdTable', 'adapterSetSearch',
                     'adapterMiddleScan',
                     'adapterMiddleScanDevice', 'pb200MiddleThresholdTable', 'adapterTrimReads', 'adapterTrimReadsDevice',
-                    'adapterTrimSplitReadsDevice', 'adapterDemuxReadsDevice', 'pb200FormatRecord', 'pb200DeviceCount', 'pb200SetDevice', 'pb200Synchronize', 'pb200LastError',
+                    'adapterTrimSplitReadsDevice', 'adapterDemuxReadsDevice', 'pb200EmitReadsDevice', 'pb200FormatRecord', 'pb200DeviceCount', 'pb200SetDevice', 'pb200Synchronize', 'pb200LastError',
                     'pb200KernelLaunches', 'pb200TimingEnable', 'pb200TimingRead', 'pb200TimingReadKinds', 'pb200SetOption',
                     'pb200GetOption', 'pb200HostBuffer', 'pb200PackNibbles']
 
@@ -558,6 +570,29 @@ def adapter_demux_reads_device(d_seqs_ptr, d_seq_off_ptr, n_seqs, total_seq_byte
         e.n_parts, e.n_out_bases, e.read_bin, e.bin_parts = n_parts.value, n_bases.value, read_bin, bin_parts
         raise
     return st, et, n_hits, hits, n_parts.value, n_bases.value, read_bin, bin_parts
+
+
+def pb200_emit_reads_device(n_rec, *, d_seq_ptr, d_qual_ptr, seq_bytes, d_off_ptr, d_read_ptr, d_part_ptr, d_names_ptr,
+                            d_name_off_ptr, n_reads, name_bytes, d_rna_ptr=0, fmt='fastq', d_out_ptr=0, out_cap=0,
+                            d_out_off_ptr=0, stream_ptr=0):
+    """The bytes Porechop writes for n_rec records in device memory (pb200EmitReadsDevice): record r is
+    seq[off[r] .. off[r + 1]) with its qualities, source read read[r] and part number part[r]; the output goes to d_out
+    (out_cap bytes) and the record byte offsets to d_out_off (int64[n_rec + 1]).  fmt: 'fastq' or 'fasta'.
+    Returns the number of bytes written.  When they do not fit out_cap it raises EngineError with code ERR_SPACE and the
+    total as .n_out_bytes (d_out_off is then valid)."""
+    if fmt not in ('fastq', 'fasta'):
+        raise ValueError("fmt must be 'fastq' or 'fasta'")
+    n_out = c_int64(0)
+    args = EmitArgsDesc(d_seq_ptr or None, d_qual_ptr or None, int(seq_bytes), d_off_ptr or None, d_read_ptr or None,
+                        d_part_ptr or None, d_names_ptr or None, d_name_off_ptr or None, int(n_reads), int(name_bytes),
+                        d_rna_ptr or None, 0 if fmt == 'fastq' else 1, d_out_ptr or None, int(out_cap), d_out_off_ptr or None,
+                        addressof(n_out))
+    try:
+        _check(C_LIB.pb200EmitReadsDevice(byref(args), int(n_rec), c_void_p(stream_ptr)))
+    except EngineError as e:
+        e.n_out_bytes = n_out.value
+        raise
+    return n_out.value
 
 
 def middle_threshold_table(middle_threshold, length):

@@ -714,16 +714,21 @@ bool single_pass_ascii(const AdapterPlan &P, int64_t max_n) {
     return true;
 }
 
-int check_status(Stage &S, cudaStream_t stream) {
-    int st = 0;
-    CK(cudaMemcpyAsync(&st, S.misc.p, 4, cudaMemcpyDeviceToHost, stream));
-    CK(cudaStreamSynchronize(stream));
+// the error a status word reports (0: none)
+int status_error(int st) {
     if (st & 1) return fail(PB200_ERR_INTERNAL, "traceback left its window (window bound violated)");
     if (st & 2) return fail(PB200_ERR_INTERNAL, "decision kernel: value outside its table (len_aln >= table length or count > 65535)");
     return 0;
 }
+int check_status(Stage &S, cudaStream_t stream) {
+    int st = 0;
+    CK(cudaMemcpyAsync(&st, S.misc.p, 4, cudaMemcpyDeviceToHost, stream));
+    CK(cudaStreamSynchronize(stream));
+    return status_error(st);
+}
 
-// S.misc: status word at offset 0, score-pass counter at 16, max-length scratch at 32.  The status word is sticky until
+// S.misc: status word at offset 0, score-pass counter at 16, max-length scratch at 32, pb200EmitReadsDevice's record-check flag
+// at 48.  The status word is sticky until
 // pb200Synchronize, which reports and clears it: a deferred error of an earlier device-resident call must not be lost, so a
 // call clears the word only when it allocates it, and everything behind it always.
 int reset_misc(Stage &S, cudaStream_t stream) {
@@ -2430,6 +2435,75 @@ int trim_reads(const uint8_t *seqs, const int64_t *seq_off, int64_t n_seqs, bool
     return 0;
 }
 
+// ---- output files (pb200EmitReadsDevice) -------------------------------------------------------------------------------
+// Record lengths (checked on the device) scanned into d_out_off; the total, the check flag and the sticky status word come home
+// in one synchronise; then, when everything holds, one warp per record writes the bytes.
+int emit_reads(const pb200_emit_args_t *A, int64_t n_rec, void *user_stream) {
+    if (!A) return fail(PB200_ERR_ARG, "NULL pointer");
+    if (A->n_out_bytes) *A->n_out_bytes = 0;
+    if (A->fmt != 0 && A->fmt != 1) return fail(PB200_ERR_ARG, "fmt must be 0 (FASTQ) or 1 (FASTA)");
+    if (A->fmt == 0 && !A->d_qual) return fail(PB200_ERR_ARG, "FASTQ needs d_qual");
+    if (n_rec < 0 || A->seq_bytes < 0 || A->n_reads < 0 || A->name_bytes < 0 || A->out_cap < 0)
+        return fail(PB200_ERR_ARG, "negative count");
+    if (!A->n_out_bytes || !A->d_out_off || (A->seq_bytes > 0 && !A->d_seq) || (A->name_bytes > 0 && !A->d_names) ||
+        (A->n_reads > 0 && !A->d_name_off) || (A->out_cap > 0 && !A->d_out) ||
+        (n_rec > 0 && (!A->d_off || !A->d_read || !A->d_part)))
+        return fail(PB200_ERR_ARG, "NULL pointer");
+
+    Engine *Ep = nullptr;
+    if (int rc = get_engine(&Ep)) return rc;
+    Engine &E = *Ep;
+    std::lock_guard<std::mutex> lk(E.mu);
+    if (int rc = E.init()) return rc;
+    Stage &S = E.st[0];
+    cudaStream_t stream = S.stream;
+    if (int rc = library_stream(E, user_stream, &stream)) return rc;
+    if (int rc = order_after_last(E, stream)) return rc;
+    NvtxRange range("pb200:emit");
+    int64_t total = 0;
+    auto run = [&]() -> int {
+        if (int rc = reset_misc(S, stream)) return rc;
+        int *bad = reinterpret_cast<int *>(S.misc.as<char>() + 48);
+        if (n_rec > 0) {
+            emit_count_kernel<<<(unsigned)((n_rec + 255) / 256), 256, 0, stream>>>(A->d_off, A->d_read, A->d_part, A->d_name_off, n_rec,
+                                                                                   A->seq_bytes, A->n_reads, A->name_bytes, A->fmt,
+                                                                                   A->d_out_off, bad);
+            g_launches++;
+            CK(cudaGetLastError());
+            if (int rc = scan_offsets(E, stream, A->d_out_off, n_rec)) return rc;
+        } else {
+            CK(cudaMemsetAsync(A->d_out_off, 0, 8, stream));
+        }
+        int st[2] = {0, 0};
+        CK(cudaMemcpyAsync(&total, A->d_out_off + n_rec, 8, cudaMemcpyDeviceToHost, stream));
+        CK(cudaMemcpyAsync(&st[0], S.misc.p, 4, cudaMemcpyDeviceToHost, stream));
+        CK(cudaMemcpyAsync(&st[1], bad, 4, cudaMemcpyDeviceToHost, stream));
+        CK(cudaStreamSynchronize(stream));
+        *A->n_out_bytes = total;
+        if (int rc = status_error(st[0])) return rc;       // a deferred error of an earlier device-resident call
+        if (st[1]) return fail(PB200_ERR_ARG, "a record's offsets, read, part or name range is out of range");
+        if (total > A->out_cap) return fail(PB200_ERR_SPACE, "out_cap is smaller than the output (*n_out_bytes)");
+        if (n_rec > 0) {
+            const int64_t blocks = std::max<int64_t>(1, std::min<int64_t>((n_rec + 7) / 8, (int64_t)E.sm_count * 8));
+            emit_write_kernel<<<(unsigned)blocks, 256, 0, stream>>>(A->d_seq, A->d_qual, A->d_off, A->d_read, A->d_part, A->d_names,
+                                                                    A->d_name_off, A->d_rna, A->fmt,
+                                                                    static_cast<const int64_t *>(A->d_out_off), n_rec, A->d_out);
+            g_launches++;
+            CK(cudaGetLastError());
+            CK(cudaStreamSynchronize(stream));              // the device outputs are written when the call returns
+        }
+        return 0;
+    };
+    const int rc = run();
+    if (rc) {                             // nothing may still be running (or writing the caller's outputs) when we return
+        const std::string first_err = g_err;
+        cudaStreamSynchronize(stream);
+        g_err = first_err;
+    }
+    E.last_pending = false;               // the stream waited for an earlier call's queued work, and all of it is done
+    return rc;
+}
+
 }  // namespace
 
 // =====================================================================================================
@@ -2511,6 +2585,11 @@ int adapterDemuxReadsDevice(const uint8_t *d_seqs, const int64_t *d_seq_off, int
     if (split->n_out_bases) *split->n_out_bases = 0;
     if (!demux) return fail(PB200_ERR_ARG, "NULL pointer");
     return trim_reads(d_seqs, d_seq_off, n_seqs, true, total_seq_bytes, max_seq_len, args, ma, mi, go, ge, stream, split, demux);
+}
+
+int pb200EmitReadsDevice(const pb200_emit_args_t *args, int64_t n_rec, void *stream) {
+    g_err.clear();
+    return emit_reads(args, n_rec, stream);
 }
 
 int pb200MiddleThresholdTable(double middle_threshold, int32_t len, int32_t *cmin) {

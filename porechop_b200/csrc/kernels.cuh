@@ -1217,13 +1217,25 @@ __global__ void split_write_kernel(PB_SPLIT_READS_PARAMS, const int64_t *rec_off
         pos += l;
     });
 }
-// dst[0 .. n) = src[0 .. n) by one warp: the bytes up to dst's next 16-byte boundary one per lane, then aligned 16-byte stores
+// Byte maps of warp_copy, applied to 32-bit words of four bytes (a single byte is a word with three zero bytes).
+struct CopyBytes {
+    __device__ __forceinline__ unsigned operator()(unsigned w) const { return w; }
+};
+struct CopyTtoU {   // every 'T' byte becomes 'U' (0x54 -> 0x55), nothing else changes: RNA reads (get_fastq / get_fasta)
+    __device__ __forceinline__ unsigned operator()(unsigned w) const {
+        const unsigned t = w ^ 0x54545454u;                                          // zero bytes where w has a 'T'
+        const unsigned nz = ((t & 0x7f7f7f7fu) + 0x7f7f7f7fu) | t;                   // high bit set in every nonzero byte
+        return w + ((~nz & 0x80808080u) >> 7);                                       // +1 in the 'T' bytes (no carry out)
+    }
+};
+// dst[0 .. n) = f(src[0 .. n)) by one warp: the bytes up to dst's next 16-byte boundary one per lane, then aligned 16-byte stores
 // assembled from aligned 16-byte loads (each lane's chunk and the next lane's, shifted into place with __funnelshift_r), then
 // the last bytes one per lane.  Loads never leave [src & ~15, src + n): the body stops where its next chunk would.
-__device__ __forceinline__ void warp_copy(const uint8_t *src, uint8_t *dst, int64_t n, int lane) {
+template <class F = CopyBytes>
+__device__ __forceinline__ void warp_copy(const uint8_t *src, uint8_t *dst, int64_t n, int lane, F f = F()) {
     int64_t h = (int64_t)((16 - ((uintptr_t)dst & 15)) & 15);
     if (h > n) h = n;
-    if (lane < h) dst[lane] = src[lane];
+    if (lane < h) dst[lane] = (uint8_t)f(src[lane]);
     const uintptr_t s1 = (uintptr_t)(src + h);
     const uint4 *A = reinterpret_cast<const uint4 *>(s1 & ~(uintptr_t)15);
     const int o = (int)(s1 & 15), q = o >> 2;
@@ -1248,11 +1260,11 @@ __device__ __forceinline__ void warp_copy(const uint8_t *src, uint8_t *dst, int6
                        t5 = q2 ? d.w : d.y;
         const unsigned u0 = q1 ? t1 : t0, u1 = q1 ? t2 : t1, u2 = q1 ? t3 : t2, u3 = q1 ? t4 : t3, u4 = q1 ? t5 : t4;
         if (v < nvec)
-            D[v] = make_uint4(__funnelshift_r(u0, u1, sh), __funnelshift_r(u1, u2, sh), __funnelshift_r(u2, u3, sh),
-                              __funnelshift_r(u3, u4, sh));
+            D[v] = make_uint4(f(__funnelshift_r(u0, u1, sh)), f(__funnelshift_r(u1, u2, sh)), f(__funnelshift_r(u2, u3, sh)),
+                              f(__funnelshift_r(u3, u4, sh)));
     }
     const int64_t t = h + 16 * nvec;                         // at most 30 bytes are left
-    if (lane < n - t) dst[t + lane] = src[t + lane];
+    if (lane < n - t) dst[t + lane] = (uint8_t)f(src[t + lane]);
 }
 // bases (and qualities) of records [0, n_rec) of the segment: source src[i], output out_off[i] .. out_off[i + 1] (out_off = the
 // caller's offsets from the segment's first record on); one warp per record
@@ -1266,6 +1278,109 @@ __global__ void __launch_bounds__(256) split_gather_kernel(const uint8_t *__rest
         const int64_t from = src[i], to = out_off[i], len = out_off[i + 1] - to;
         warp_copy(seq + from, out_seq + to, len, lane);
         if (qual) warp_copy(qual + from, out_qual + to, len, lane);
+    }
+}
+
+// ---------------------------------------------------------------------------------------------------
+// pb200EmitReadsDevice: the bytes Porechop writes for records in device memory (get_fastq / get_fasta, fastq.emit_parts).
+// Record r: bases seq[off[r] .. off[r + 1]) (qualities at the same offsets), source read read[r], part part[r] (k >= 1: '_k'
+// goes before the first space of the name, add_number_to_read_name); names[name_off[s] .. name_off[s + 1]) of read s.
+// FASTQ: '@' name '\n' bases '\n' '+' '\n' quals '\n'; FASTA: '>' name '\n' and the bases in lines of 70, each ending in '\n'.
+
+// decimal digits of k >= 1
+__device__ __forceinline__ int emit_digits(int32_t k) {
+    int d = 1;
+    for (int64_t p = 10; p <= k; p *= 10) ++d;
+    return d;
+}
+// byte length of record r, and whether its arrays are in range (checked here because they come from outside the library)
+__device__ __forceinline__ int64_t emit_record_len(int64_t sl, int64_t nl, int32_t part, int32_t fmt) {
+    const int64_t name = nl + (part > 0 ? 1 + emit_digits(part) : 0);
+    return fmt == 0 ? 6 + name + 2 * sl : 2 + name + sl + (sl + 69) / 70;
+}
+// len[r + 1] = byte length of record r (len[0] = 0), for scan_offsets; a record that fails a check gets length 0 and sets
+// *bad.  One thread per record.
+__global__ void emit_count_kernel(const int64_t *off, const int32_t *read, const int32_t *part, const int64_t *name_off,
+                                  int64_t n_rec, int64_t seq_bytes, int64_t n_reads, int64_t name_bytes, int32_t fmt, int64_t *len,
+                                  int *bad) {
+    const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (r == 0) len[0] = 0;
+    if (r >= n_rec) return;
+    const int64_t a = off[r], b = off[r + 1];
+    const int32_t s = read[r], k = part[r];
+    bool ok = 0 <= a && a <= b && b <= seq_bytes && 0 <= s && s < n_reads && k >= 0;
+    int64_t nl = 0;
+    if (ok) {
+        const int64_t n0 = name_off[s], n1 = name_off[s + 1];
+        ok = 0 <= n0 && n0 <= n1 && n1 <= name_bytes;
+        nl = n1 - n0;
+    }
+    if (!ok) atomicOr(bad, 1);
+    len[r + 1] = ok ? emit_record_len(b - a, nl, k, fmt) : 0;
+}
+// the records at out + out_off[r] (scanned by emit_count_kernel + scan_offsets; every check passed); one warp per record.
+// Names and the FASTA lines go one byte per lane; FASTQ bases and qualities through warp_copy.
+__global__ void __launch_bounds__(256) emit_write_kernel(const uint8_t *seq, const uint8_t *qual, const int64_t *off,
+                                                         const int32_t *read, const int32_t *part, const uint8_t *names,
+                                                         const int64_t *name_off, const uint8_t *rna, int32_t fmt,
+                                                         const int64_t *out_off, int64_t n_rec, uint8_t *out) {
+    const int lane = threadIdx.x & 31;
+    const int64_t warps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    for (int64_t r = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; r < n_rec; r += warps) {
+        const int64_t s0 = off[r], sl = off[r + 1] - s0;
+        const int32_t s = read[r], k = part[r];
+        const int64_t n0 = name_off[s], nl = name_off[s + 1] - n0;
+        const uint8_t *nm = names + n0;
+        uint8_t *p = out + out_off[r];
+        // ---- the name: the tag '_k' (td bytes) goes at sp, the first space (or the end) ----
+        int td = 0;
+        int64_t sp = nl;
+        if (k > 0) {
+            td = 1 + emit_digits(k);
+            for (int64_t c = 0; c < nl; c += 32) {                // warp-uniform: 32 name bytes a step
+                const int64_t j = c + lane;
+                const int first = __reduce_min_sync(0xffffffffu, (j < nl && nm[j] == ' ') ? lane : 32);
+                if (first < 32) { sp = c + first; break; }
+            }
+        }
+        if (lane == 0) p[0] = fmt == 0 ? '@' : '>';
+        const int64_t L = nl + td;
+        for (int64_t j = lane; j < L; j += 32) {
+            uint8_t v;
+            if (j < sp) v = nm[j];
+            else if (j >= sp + td) v = nm[j - td];
+            else if (j == sp) v = '_';
+            else {                                                 // digit q of k, most significant first
+                int64_t div = 1;
+                for (int64_t q = j - sp; q < td - 1; ++q) div *= 10;
+                v = (uint8_t)('0' + (k / div) % 10);
+            }
+            p[1 + j] = v;
+        }
+        if (lane == 0) p[1 + L] = '\n';
+        uint8_t *b = p + 2 + L;
+        const bool u = rna && rna[s];
+        if (fmt == 0) {
+            if (u) warp_copy(seq + s0, b, sl, lane, CopyTtoU());
+            else warp_copy(seq + s0, b, sl, lane);
+            warp_copy(qual + s0, b + sl + 3, sl, lane);
+            if (lane == 0) { b[sl] = '\n'; b[sl + 1] = '+'; b[sl + 2] = '\n'; b[2 * sl + 3] = '\n'; }
+        } else {
+            // output byte j of the base lines is column c of line l (71 bytes a line: 70 bases and '\n'); a lane moves 32 bytes
+            // a step, so (l, c) follow without a division
+            const int64_t nb = sl + (sl + 69) / 70;
+            int64_t l = 0, c = lane;
+            for (int64_t j = lane; j < nb; j += 32) {
+                uint8_t v = '\n';
+                if (c < 70 && j != nb - 1) {
+                    v = seq[s0 + 70 * l + c];
+                    if (u && v == 'T') v = 'U';
+                }
+                b[j] = v;
+                c += 32;
+                if (c >= 71) { c -= 71; ++l; }
+            }
+        }
     }
 }
 

@@ -1,17 +1,22 @@
 """
-Porechop on reads that are already in GPU memory: trimmed and split output reads, with their qualities, in GPU memory.
+Porechop on reads that are already in GPU memory: trimmed and split output reads, with their qualities, and the bytes of
+Porechop's output files, in GPU memory.
 
 For callers whose reads live on the device (a basecaller on the same card, a torch pipeline): one
 adapterTrimSplitReadsDevice call runs Phase B (end trims), Phase C (middle adapters) and cuts the records Porechop writes --
 the records fastq.emit would write for the same decisions, in the same order -- into device tensors.  Only the decisions
-(trims, hits, barcode rankings) come to the host; the bases and qualities never do.
+(trims, hits, barcode rankings) come to the host; the bases and qualities never do.  emit_reads (pb200EmitReadsDevice) then
+formats the records on the device -- the bytes fastq.emit_parts writes: numbered names of split parts, U for RNA reads,
+70-column FASTA -- so that the file's bytes come home in one copy:
 
-    from porechop_b200 import device_reads, fastq
+    import torch
+    from porechop_b200 import device_reads
     out = device_reads.trim_reads(seq, seq_off, matching_sets, (3, -6, -5, -2), qual)
     # out.seq / out.qual / out.off / out.read / out.part: CUDA tensors; record r is seq[off[r]:off[r+1]] of read read[r],
-    # part[r] = 0 (not split) or k >= 1 (the k-th part).  To write files:
-    data = fastq.emit_parts(name_buf, name_off, rna, tuple(x.cpu().numpy() if x is not None else None
-                                                           for x in out[:5]), 'fastq')
+    # part[r] = 0 (not split) or k >= 1 (the k-th part).  names / name_off: the reads' names as CUDA tensors (uint8, int64).
+    em = device_reads.emit_reads(out, names, name_off, rna, 'fastq')
+    data = torch.empty(em.data.numel(), dtype=torch.uint8, pin_memory=True).copy_(em.data)
+    open('out.fastq', 'wb').write(data.numpy())
 
 demux_reads does the same for `porechop -b DIR`: it also calls every read's barcode on the device and returns the records
 grouped by bin, so that each bin's reads are one contiguous slice of records and bytes:
@@ -19,9 +24,10 @@ grouped by bin, so that each bin's reads are one contiguous slice of records and
     out = device_reads.demux_reads(seq, seq_off, matching_sets, (3, -6, -5, -2), qual, forward_or_reverse='forward',
                                    barcode_threshold=75.0, barcode_diff=5.0, require_two_barcodes=False,
                                    discard_unassigned=False)
-    for name, (r0, r1) in out.bins.items():          # the bytes demux_fastq writes into <name>.fastq
-        parts = (out.seq, out.qual, out.off[r0:r1 + 1], out.read[r0:r1], out.part[r0:r1])
-        data = fastq.emit_parts(name_buf, name_off, rna, tuple(x.cpu().numpy() for x in parts), 'fastq')
+    em = device_reads.emit_reads(out, names, name_off, rna, 'fastq')
+    data = torch.empty(em.data.numel(), dtype=torch.uint8, pin_memory=True).copy_(em.data)
+    for name, (b0, b1) in em.bins.items():           # the bytes demux_fastq writes into <name>.fastq
+        open(name + '.fastq', 'wb').write(data[b0:b1].numpy())
 
 The device work runs on torch.cuda.current_stream(); the call returns when the outputs are written.  `W` (the engine's
 wrapper module) and `device()` (the allocator) are module attributes, so that the same set handling and retry logic can run
@@ -36,6 +42,7 @@ from . import fastq
 
 TrimmedReads = collections.namedtuple('TrimmedReads', 'seq qual off read part start_trim end_trim hits calls')
 DemuxedReads = collections.namedtuple('DemuxedReads', 'seq qual off read part bins calls start_trim end_trim hits')
+EmittedReads = collections.namedtuple('EmittedReads', 'data off bins')
 
 
 class TorchDevice:
@@ -64,6 +71,9 @@ class TorchDevice:
     def upload(self, arr):
         return self.torch.from_numpy(np.ascontiguousarray(arr)).to('cuda')
 
+    def host(self, t):
+        return t.cpu().numpy()
+
     def check(self, seq, seq_off, qual):
         torch = self.torch
         for name, t, dt in (('seq', seq, torch.uint8), ('seq_off', seq_off, torch.int64), ('qual', qual, torch.uint8)):
@@ -73,6 +83,15 @@ class TorchDevice:
                 raise ValueError('%s must be a contiguous 1-D %s CUDA tensor' % (name, dt))
         if qual is not None and qual.numel() != seq.numel():
             raise ValueError('qual must hold one quality per base, at the offsets of the reads')
+
+    def check_names(self, names, name_off, rna):
+        torch = self.torch
+        for name, t, dts in (('names', names, (torch.uint8,)), ('name_off', name_off, (torch.int64,)),
+                             ('rna', rna, (torch.bool, torch.uint8))):
+            if t is None:
+                continue
+            if not (t.is_cuda and t.dtype in dts and t.dim() == 1 and t.is_contiguous()):
+                raise ValueError('%s must be a contiguous 1-D %s CUDA tensor' % (name, ' or '.join(str(d) for d in dts)))
 
 
 _device = None
@@ -210,3 +229,54 @@ def demux_reads(seq, seq_off, matching_sets, scoring_scheme_vals, qual=None, *, 
     return DemuxedReads(D.head(out_seq, n_out), D.head(out_qual, n_out) if out_qual is not None else None,
                         D.head(out_off, n_parts + 1), D.head(out_read, n_parts), D.head(out_part, n_parts), bins,
                         [bin_names[b] for b in read_bin.tolist()], st, et, fastq._hits_dict(n_hits, h))
+
+
+def initial_out_cap(n_rec, n_bases, longest_name, fmt):
+    """room for the output bytes of the first attempt: an upper bound -- the bases (and qualities), then per record the longest
+    name, an 11-byte part tag ('_' and up to 10 digits) and the fixed bytes (FASTQ '@', '\\n', '\\n+\\n', '\\n'; FASTA '>', '\\n'
+    and at most one more line end than n_bases / 70)"""
+    if fmt == 'fastq':
+        return 2 * n_bases + n_rec * (longest_name + 11 + 6)
+    return n_bases + n_bases // 70 + n_rec * (longest_name + 11 + 3)
+
+
+def emit_reads(out, names, name_off, rna=None, fmt='fastq'):
+    """The bytes Porechop writes for the records of trim_reads / demux_reads (a TrimmedReads or DemuxedReads), formatted on the
+    device (pb200EmitReadsDevice): the bytes fastq.emit_parts writes for the same records.  names (uint8) / name_off
+    (int64[n_reads + 1]): the source reads' names; rna: bool or uint8 per read (RNA reads are written with U), or None.
+    fmt: 'fastq' or 'fasta'.
+    Returns EmittedReads: data (uint8, exactly the output's length) and off (int64[n_records + 1], record byte offsets) on the
+    device; bins = {name: (first byte, end byte)} of every bin of a DemuxedReads -- each bin's file is one slice of data --
+    or None for a TrimmedReads."""
+    if fmt not in ('fastq', 'fasta'):
+        raise ValueError("fmt must be 'fastq' or 'fasta'")
+    if fmt == 'fastq' and out.qual is None:
+        raise ValueError('FASTQ output needs the qualities')
+    D = device()
+    if hasattr(D, 'check_names'):
+        D.check_names(names, name_off, rna)
+    n_rec, n_reads = D.numel(out.read), D.numel(name_off) - 1
+    if n_reads < 0 or (rna is not None and D.numel(rna) != n_reads):
+        raise ValueError('name_off needs n_reads + 1 offsets and rna one flag per read')
+    name_len = np.diff(D.host(name_off))
+    cap = initial_out_cap(n_rec, D.numel(out.seq), int(name_len.max()) if len(name_len) else 0, fmt)
+    off = D.empty(n_rec + 1, np.int64)
+    for attempt in range(2):
+        data = D.empty(max(cap, 1), np.uint8)
+        try:
+            n_out = W.pb200_emit_reads_device(
+                n_rec, d_seq_ptr=D.ptr(out.seq), d_qual_ptr=D.ptr(out.qual) if fmt == 'fastq' else 0, seq_bytes=D.numel(out.seq),
+                d_off_ptr=D.ptr(out.off), d_read_ptr=D.ptr(out.read), d_part_ptr=D.ptr(out.part), d_names_ptr=D.ptr(names),
+                d_name_off_ptr=D.ptr(name_off), n_reads=n_reads, name_bytes=D.numel(names), d_rna_ptr=D.ptr(rna), fmt=fmt,
+                d_out_ptr=D.ptr(data), out_cap=cap, d_out_off_ptr=D.ptr(off), stream_ptr=D.stream())
+        except W.EngineError as e:
+            if e.code == W.ERR_SPACE and attempt == 0 and getattr(e, 'n_out_bytes', 0) > cap:
+                cap = e.n_out_bytes                   # the exact number of bytes: one more call
+                continue
+            raise
+        break
+    bins = None
+    if isinstance(out, DemuxedReads):
+        o = D.host(off)
+        bins = {name: (int(o[r0]), int(o[r1])) for name, (r0, r1) in out.bins.items()}
+    return EmittedReads(D.head(data, n_out), off, bins)

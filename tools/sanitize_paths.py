@@ -120,6 +120,14 @@ def split_reads():
     r = device_reads.trim_reads(torch.from_numpy(lbuf).cuda(), torch.from_numpy(loff).cuda(), sets, wl.DEFAULT_SCORING,
                                 torch.from_numpy(qual).cuda(), min_split_read_size=100)
     got = fastq.emit_parts(names, name_off, rna, tuple(x.cpu().numpy() for x in r[:5]), 'fastq')
+    # the same records formatted on the device (pb200EmitReadsDevice), in both formats
+    d_names = [torch.from_numpy(x).cuda() for x in (names, name_off, rna)]
+    for fmt in ('fastq', 'fasta'):
+        em = device_reads.emit_reads(r, *d_names, fmt)
+        parts = tuple(x.cpu().numpy() for x in r[:5])
+        if em.data.cpu().numpy().tobytes() != fastq.emit_parts(names, name_off, rna, parts if fmt == 'fastq' else
+                                                               (parts[0], None) + parts[2:], fmt):
+            return np.zeros(1), np.ones(1)
     st, et, _, _, n_hits, h = W.adapter_trim_reads(lbuf, loff, sides[0], sides[1], (a2, o2), wl.DEFAULT_SCORING, 150, 2, 75.0, 4, 85.0)
     middle = fastq.middle_trim_ranges(fastq._hits_dict(n_hits, h), [('t', yt), ('b', yb)], {'t'}, {'b'}, 10, 100)
     batch = fastq.FastqBatch(names, name_off, lbuf, loff, qual, loff, rna)
@@ -147,7 +155,10 @@ def demux_reads():
     r = device_reads.demux_reads(torch.from_numpy(buf).cuda(), torch.from_numpy(off).cuda(), sets, wl.DEFAULT_SCORING,
                                  torch.from_numpy(qual).cuda(), min_split_read_size=100, **bc)
     parts = tuple(x.cpu().numpy() for x in r[:5])
-    got = b''.join(fastq.emit_parts(names, name_off, batch.rna, parts[:2] + (parts[2][r0:r1 + 1], parts[3][r0:r1],
+    em = device_reads.emit_reads(r, *(torch.from_numpy(x).cuda() for x in (names, name_off, batch.rna)), 'fastq')
+    data = em.data.cpu().numpy().tobytes()
+    got = b''.join(data[b0:b1] for b0, b1 in em.bins.values())
+    assert got == b''.join(fastq.emit_parts(names, name_off, batch.rna, parts[:2] + (parts[2][r0:r1 + 1], parts[3][r0:r1],
                                                                             parts[4][r0:r1]), 'fastq') for r0, r1 in r.bins.values())
     bins, _ = fastq.demux_fastq(batch, sets, wl.DEFAULT_SCORING, min_split_read_size=100, **bc)
     exp = b''.join(bins[k] for k in r.bins) if sorted(bins) == sorted(r.bins) else b''
