@@ -311,6 +311,42 @@ int get_engine(Engine **out) {
     return 0;
 }
 
+// Where an entry point runs: st[0]; the library stream of a device-resident call (library_stream); or st[0] with every
+// stage's stream waiting for earlier queued work (the calls that run the chunk pipeline, run_cross_jobs, on all stages).
+enum class CallOn { stage0, library, stages };
+
+// The engine of the current device, locked and initialised, and the call's stream ordered after the work earlier calls left
+// queued; then body(E, stream).
+template <class Body>
+int with_engine(CallOn on, void *user_stream, Body &&body) {
+    Engine *Ep = nullptr;
+    if (int rc = get_engine(&Ep)) return rc;
+    Engine &E = *Ep;
+    std::lock_guard<std::mutex> lk(E.mu);
+    if (int rc = E.init()) return rc;
+    cudaStream_t stream = E.st[0].stream;
+    if (on == CallOn::library) { if (int rc = library_stream(E, user_stream, &stream)) return rc; }
+    if (int rc = on == CallOn::stages ? order_stages_after_last(E) : order_after_last(E, stream)) return rc;
+    return body(E, stream);
+}
+
+// with_engine for a call that returns with its work done: when the body fails, nothing may still be running (or reading and
+// writing the caller's buffers) when the call returns, so the stream is drained, keeping the first error's message.  Either
+// way the stream has waited for the earlier calls' queued work, and all of it is done.
+template <class Body>
+int sync_call(CallOn on, void *user_stream, Body &&body) {
+    return with_engine(on, user_stream, [&](Engine &E, cudaStream_t stream) -> int {
+        const int rc = body(E, stream);
+        if (rc) {
+            const std::string first_err = g_err;
+            cudaStreamSynchronize(stream);
+            g_err = first_err;
+        }
+        E.last_pending = false;
+        return rc;
+    });
+}
+
 // ---- int16 domain checks and the window bound ------------------------------------------------------------
 struct SchemeInfo {
     bool int16_ok_base;   // sign conventions allow the packed kernels at all
@@ -613,14 +649,27 @@ int plan_adapters(Engine &E, cudaStream_t stream, const uint8_t *adapters, const
     return 0;
 }
 
-// Generic (int32) class: jobs are planned on the host, which needs the sequence lengths there.
-int run_generic_cross(Engine &E, Stage &S, cudaStream_t stream, const ClassPlan &C, const int64_t *h_seq_off,
-                      int64_t s0, int64_t cnt, int64_t base_off, const int32_t *h_ad_off, int32_t n_adapters,
-                      const uint8_t *seq_codes, const uint8_t *ad_codes, const Scoring &sc, int32_t *out) {
+// Alignments of the generic (int32) class, planned on the host (which needs the sequence lengths there) and batched so that
+// a batch's trace matrices fit a 2 GiB scratch: one generic_kernel launch per batch, waited for before the scratch is reused.
+// The last batch runs at flush().
+struct GenericBatch {
+    Engine &E;
+    cudaStream_t stream;
+    const uint8_t *seq_codes, *ad_codes;
+    const Scoring &sc;
+    int32_t *out;
     std::vector<GenericJob> jobs;
-    const size_t budget = 2ull << 30;
     size_t used = 0;
-    auto flush = [&]() -> int {
+    int add(int64_t seq_off, int32_t n, int32_t m, int32_t ad_off, int32_t out_idx) {
+        size_t tb = (((size_t)(n + 1) * (size_t)(m + 1) + 3) & ~(size_t)3) + (size_t)(m + 1) * 8;
+        tb = (tb + 15) & ~(size_t)15;
+        if (tb > (64ull << 30)) return fail(PB200_ERR_ARG, "alignment too large for the generic int32 path");
+        if (used + tb > (2ull << 30) && !jobs.empty()) { if (int rc = flush()) return rc; }
+        jobs.push_back(GenericJob{seq_off, n, m, ad_off, out_idx, (int64_t)used});
+        used += tb;
+        return 0;
+    }
+    int flush() {
         if (jobs.empty()) return 0;
         if (int rc = E.gjobs.ensure(jobs.size() * sizeof(GenericJob))) return rc;
         if (int rc = E.gscratch.ensure(used + 64)) return rc;
@@ -633,25 +682,18 @@ int run_generic_cross(Engine &E, Stage &S, cudaStream_t stream, const ClassPlan 
         CK(cudaStreamSynchronize(stream));
         jobs.clear(); used = 0;
         return 0;
-    };
-    for (int64_t s = s0; s < s0 + cnt; ++s) {
-        for (int32_t a : C.ad_ids) {
-            GenericJob j;
-            j.seq_off = h_seq_off[s] - base_off;
-            j.n = (int32_t)(h_seq_off[s + 1] - h_seq_off[s]);
-            j.m = h_ad_off[a + 1] - h_ad_off[a];
-            j.ad_off = h_ad_off[a];
-            j.out_idx = (int32_t)((s - s0) * n_adapters + a);
-            size_t tb = (((size_t)(j.n + 1) * (size_t)(j.m + 1) + 3) & ~(size_t)3) + (size_t)(j.m + 1) * 8;
-            tb = (tb + 15) & ~(size_t)15;
-            if (tb > (64ull << 30)) return fail(PB200_ERR_ARG, "alignment too large for the generic int32 path");
-            if (used + tb > budget && !jobs.empty()) { if (int rc = flush()) return rc; }
-            j.scratch_off = (int64_t)used;
-            used += tb;
-            jobs.push_back(j);
-        }
     }
-    return flush();
+};
+
+int run_generic_cross(Engine &E, cudaStream_t stream, const ClassPlan &C, const int64_t *h_seq_off, int64_t s0, int64_t cnt,
+                      int64_t base_off, const int32_t *h_ad_off, int32_t n_adapters, const uint8_t *seq_codes,
+                      const uint8_t *ad_codes, const Scoring &sc, int32_t *out) {
+    GenericBatch G{E, stream, seq_codes, ad_codes, sc, out};
+    for (int64_t s = s0; s < s0 + cnt; ++s)
+        for (int32_t a : C.ad_ids)
+            if (int rc = G.add(h_seq_off[s] - base_off, (int32_t)(h_seq_off[s + 1] - h_seq_off[s]), h_ad_off[a + 1] - h_ad_off[a],
+                               h_ad_off[a], (int32_t)((s - s0) * n_adapters + a))) return rc;
+    return G.flush();
 }
 
 // Cross product of sequences [s0, s0+cnt) (already encoded on the device, offsets on the device) with all adapters.
@@ -687,7 +729,7 @@ int run_cross_chunk(Engine &E, Stage &S, cudaStream_t stream, const AdapterPlan 
         if (C.cls == GENERIC_CLASS) {
             if (!h_seq_off_abs) return fail(PB200_ERR_INTERNAL, "generic class needs host offsets");
             if (seq_ascii) return fail(PB200_ERR_INTERNAL, "ASCII sequences reached the generic class");
-            if (int rc = run_generic_cross(E, S, stream, C, h_seq_off_abs, s0, cnt, base_off, h_ad_off, n_adapters, seq_codes,
+            if (int rc = run_generic_cross(E, stream, C, h_seq_off_abs, s0, cnt, base_off, h_ad_off, n_adapters, seq_codes,
                                            P.d_ad_codes, P.sc, d_out)) return rc;
             continue;
         }
@@ -1189,125 +1231,83 @@ int batch_host(const uint8_t *seqs, const int64_t *seq_off, int64_t n_seqs, cons
     std::vector<CrossJob> jobs(1);
     jobs[0] = CrossJob{seqs, seq_off, n_seqs, adapters, ad_off, n_adapters, out};
     if (int rc = validate_args(seqs, seq_off, n_seqs, adapters, ad_off, n_adapters, pair_seq, pair_adapter, n_pairs, cross)) return rc;
-    Engine *Ep = nullptr;
-    if (int rc = get_engine(&Ep)) return rc;
-    Engine &E = *Ep;
-    std::lock_guard<std::mutex> lk(E.mu);
-    if (int rc = E.init()) return rc;
-    if (cross) {
-        if (int rc = order_stages_after_last(E)) return rc;
-        return run_cross_jobs(E, jobs, ma, mi, go, ge);
-    }
-    // pair-list mode runs on st[0] alone
-    if (int rc = order_after_last(E, E.st[0].stream)) return rc;
-    AdapterPlan P;
-    if (int rc = plan_adapters(E, E.st[0].stream, adapters, ad_off, n_adapters, ma, mi, go, ge, P)) return rc;
+    if (cross)
+        return with_engine(CallOn::stages, nullptr, [&](Engine &E, cudaStream_t) { return run_cross_jobs(E, jobs, ma, mi, go, ge); });
 
-    // ---- pair-list mode: all sequences resident, pairs ordered per class on the host ----
-    auto run_pairs = [&]() -> int {
-    NvtxRange submit_range("pb200:submit_pairs");
-    Stage &S = E.st[0];
-    cudaStream_t stream = S.stream;
-    const int64_t bytes = seq_off[n_seqs];
-    if (int rc = S.seq_raw.ensure((size_t)bytes + 16)) return rc;
-    if (int rc = S.seq_codes.ensure((size_t)bytes + 16)) return rc;
-    if (int rc = S.seq_off.ensure((size_t)(n_seqs + 1) * 8)) return rc;
-    if (int rc = S.out.ensure((size_t)n_pairs * PB_REC * 4)) return rc;
-    if (int rc = S.pair_seq.ensure((size_t)n_pairs * 4)) return rc;
-    if (int rc = S.pair_ad.ensure((size_t)n_pairs * 4)) return rc;
-    if (int rc = S.order.ensure((size_t)n_pairs * 4)) return rc;
-    if (int rc = reset_misc(S, stream)) return rc;
-    if (bytes) CK(cudaMemcpyAsync(S.seq_raw.p, seqs, (size_t)bytes, cudaMemcpyHostToDevice, stream));
-    CK(cudaMemcpyAsync(S.seq_off.p, seq_off, (size_t)(n_seqs + 1) * 8, cudaMemcpyHostToDevice, stream));
-    CK(cudaMemcpyAsync(S.pair_seq.p, pair_seq, (size_t)n_pairs * 4, cudaMemcpyHostToDevice, stream));
-    CK(cudaMemcpyAsync(S.pair_ad.p, pair_adapter, (size_t)n_pairs * 4, cudaMemcpyHostToDevice, stream));
-    if (int rc = launch_encode(stream, S.seq_raw.as<uint8_t>(), S.seq_codes.as<uint8_t>(), bytes, E.sm_count)) return rc;
-    // class of every adapter, then per-class ordering (adapter, length) so that slot halves have similar shapes
-    std::vector<int> ad_class(n_adapters);
-    for (int a = 0; a < n_adapters; ++a) ad_class[a] = class_of(P.si, ad_off[a + 1] - ad_off[a]);
-    std::vector<std::vector<int32_t>> per_class(N_CLASSES);
-    for (int64_t p = 0; p < n_pairs; ++p) per_class[ad_class[pair_adapter[p]]].push_back((int32_t)p);
-    int *status = S.misc.as<int>();
-    unsigned long long *counter = reinterpret_cast<unsigned long long *>(S.misc.as<char>() + 16);
-    for (int c = 0; c < N_CLASSES; ++c) {
-        auto &ord = per_class[c];
-        if (ord.empty()) continue;
-        int m_max = 0;
-        int64_t max_n = 0;
-        for (int32_t p : ord) {
-            m_max = std::max(m_max, ad_off[pair_adapter[p] + 1] - ad_off[pair_adapter[p]]);
-            max_n = std::max(max_n, seq_off[pair_seq[p] + 1] - seq_off[pair_seq[p]]);
-        }
-        if (max_n > 0x7fff0000ll) return fail(PB200_ERR_ARG, "sequence longer than 2^31");
-        if (c == GENERIC_CLASS) {
-            // generic: reuse the cross helper one pair at a time through a tiny job list
-            std::vector<GenericJob> jobs;
-            size_t used = 0;
-            const size_t budget = 2ull << 30;
-            auto flush = [&]() -> int {
-                if (jobs.empty()) return 0;
-                if (int rc = E.gjobs.ensure(jobs.size() * sizeof(GenericJob))) return rc;
-                if (int rc = E.gscratch.ensure(used + 64)) return rc;
-                CK(cudaMemcpyAsync(E.gjobs.p, jobs.data(), jobs.size() * sizeof(GenericJob), cudaMemcpyHostToDevice, stream));
-                int nb = (int)((jobs.size() + 63) / 64);
-                generic_kernel<<<nb, 64, 0, stream>>>(E.gjobs.as<GenericJob>(), (int)jobs.size(), S.seq_codes.as<uint8_t>(),
-                                                      P.d_ad_codes, ma, mi, go, ge, E.gscratch.as<uint8_t>(),
-                                                      S.out.as<int32_t>());
-                g_launches++;
-                CK(cudaGetLastError());
-                CK(cudaStreamSynchronize(stream));
-                jobs.clear(); used = 0;
-                return 0;
-            };
+    // ---- pair-list mode: all sequences resident on st[0], pairs ordered per class on the host ----
+    return sync_call(CallOn::stage0, nullptr, [&](Engine &E, cudaStream_t stream) -> int {
+        AdapterPlan P;
+        if (int rc = plan_adapters(E, stream, adapters, ad_off, n_adapters, ma, mi, go, ge, P)) return rc;
+        NvtxRange submit_range("pb200:submit_pairs");
+        Stage &S = E.st[0];
+        const int64_t bytes = seq_off[n_seqs];
+        if (int rc = S.seq_raw.ensure((size_t)bytes + 16)) return rc;
+        if (int rc = S.seq_codes.ensure((size_t)bytes + 16)) return rc;
+        if (int rc = S.seq_off.ensure((size_t)(n_seqs + 1) * 8)) return rc;
+        if (int rc = S.out.ensure((size_t)n_pairs * PB_REC * 4)) return rc;
+        if (int rc = S.pair_seq.ensure((size_t)n_pairs * 4)) return rc;
+        if (int rc = S.pair_ad.ensure((size_t)n_pairs * 4)) return rc;
+        if (int rc = S.order.ensure((size_t)n_pairs * 4)) return rc;
+        if (int rc = reset_misc(S, stream)) return rc;
+        if (bytes) CK(cudaMemcpyAsync(S.seq_raw.p, seqs, (size_t)bytes, cudaMemcpyHostToDevice, stream));
+        CK(cudaMemcpyAsync(S.seq_off.p, seq_off, (size_t)(n_seqs + 1) * 8, cudaMemcpyHostToDevice, stream));
+        CK(cudaMemcpyAsync(S.pair_seq.p, pair_seq, (size_t)n_pairs * 4, cudaMemcpyHostToDevice, stream));
+        CK(cudaMemcpyAsync(S.pair_ad.p, pair_adapter, (size_t)n_pairs * 4, cudaMemcpyHostToDevice, stream));
+        if (int rc = launch_encode(stream, S.seq_raw.as<uint8_t>(), S.seq_codes.as<uint8_t>(), bytes, E.sm_count)) return rc;
+        // class of every adapter, then per-class ordering (adapter, length) so that slot halves have similar shapes
+        std::vector<int> ad_class(n_adapters);
+        for (int a = 0; a < n_adapters; ++a) ad_class[a] = class_of(P.si, ad_off[a + 1] - ad_off[a]);
+        std::vector<std::vector<int32_t>> per_class(N_CLASSES);
+        for (int64_t p = 0; p < n_pairs; ++p) per_class[ad_class[pair_adapter[p]]].push_back((int32_t)p);
+        int *status = S.misc.as<int>();
+        unsigned long long *counter = reinterpret_cast<unsigned long long *>(S.misc.as<char>() + 16);
+        for (int c = 0; c < N_CLASSES; ++c) {
+            auto &ord = per_class[c];
+            if (ord.empty()) continue;
+            int m_max = 0;
+            int64_t max_n = 0;
             for (int32_t p : ord) {
-                GenericJob j;
-                int64_t s = pair_seq[p]; int a = pair_adapter[p];
-                j.seq_off = seq_off[s]; j.n = (int32_t)(seq_off[s + 1] - seq_off[s]);
-                j.m = ad_off[a + 1] - ad_off[a]; j.ad_off = ad_off[a]; j.out_idx = p;
-                size_t tb = (((size_t)(j.n + 1) * (size_t)(j.m + 1) + 3) & ~(size_t)3) + (size_t)(j.m + 1) * 8;
-                tb = (tb + 15) & ~(size_t)15;
-                if (tb > (64ull << 30)) return fail(PB200_ERR_ARG, "alignment too large for the generic int32 path");
-                if (used + tb > budget && !jobs.empty()) { if (int rc = flush()) return rc; }
-                j.scratch_off = (int64_t)used; used += tb;
-                jobs.push_back(j);
+                m_max = std::max(m_max, ad_off[pair_adapter[p] + 1] - ad_off[pair_adapter[p]]);
+                max_n = std::max(max_n, seq_off[pair_seq[p] + 1] - seq_off[pair_seq[p]]);
             }
-            if (int rc = flush()) return rc;
-            continue;
+            if (max_n > 0x7fff0000ll) return fail(PB200_ERR_ARG, "sequence longer than 2^31");
+            if (c == GENERIC_CLASS) {
+                GenericBatch G{E, stream, S.seq_codes.as<uint8_t>(), P.d_ad_codes, P.sc, S.out.as<int32_t>()};
+                for (int32_t p : ord) {
+                    const int64_t s = pair_seq[p];
+                    const int a = pair_adapter[p];
+                    if (int rc = G.add(seq_off[s], (int32_t)(seq_off[s + 1] - seq_off[s]), ad_off[a + 1] - ad_off[a], ad_off[a], p))
+                        return rc;
+                }
+                if (int rc = G.flush()) return rc;
+                continue;
+            }
+            std::sort(ord.begin(), ord.end(), [&](int32_t x, int32_t y) {
+                int ax = pair_adapter[x], ay = pair_adapter[y];
+                if (ax != ay) return ax < ay;
+                int64_t nx = seq_off[pair_seq[x] + 1] - seq_off[pair_seq[x]], ny = seq_off[pair_seq[y] + 1] - seq_off[pair_seq[y]];
+                if (nx != ny) return nx < ny;
+                return x < y;
+            });
+            const int64_t n_tasks = (int64_t)ord.size();
+            if (int rc = S.tasks.ensure((size_t)n_tasks * sizeof(Task))) return rc;
+            CK(cudaMemcpyAsync(S.order.p, ord.data(), (size_t)n_tasks * 4, cudaMemcpyHostToDevice, stream));
+            CK(cudaStreamSynchronize(stream));  // ord is pageable and reused per class
+            build_tasks_pairs_kernel<<<(unsigned)((n_tasks + 255) / 256), 256, 0, stream>>>(
+                S.tasks.as<Task>(), n_tasks, S.order.as<int32_t>(), S.pair_seq.as<int32_t>(), S.pair_ad.as<int32_t>(),
+                S.seq_off.as<int64_t>(), P.d_ad_off);
+            g_launches++;
+            CK(cudaGetLastError());
+            TaskSrc ts;
+            ts.tasks = S.tasks.as<Task>(); ts.n_tasks = n_tasks;
+            ts.cls_ad = nullptr; ts.n_cls_ad = 0; ts.n_adapters = n_adapters; ts.n_seqs = n_seqs;
+            ts.seq_off = S.seq_off.as<int64_t>(); ts.ad_off = P.d_ad_off; ts.seq_order = nullptr;
+            if (int rc = run_class_tasks(E, S, stream, c, m_max, ts, max_n, S.seq_codes.as<uint8_t>(), P.d_ad_codes,
+                                         P.sc, P.si, S.out.as<int32_t>(), status, counter)) return rc;
         }
-        std::sort(ord.begin(), ord.end(), [&](int32_t x, int32_t y) {
-            int ax = pair_adapter[x], ay = pair_adapter[y];
-            if (ax != ay) return ax < ay;
-            int64_t nx = seq_off[pair_seq[x] + 1] - seq_off[pair_seq[x]], ny = seq_off[pair_seq[y] + 1] - seq_off[pair_seq[y]];
-            if (nx != ny) return nx < ny;
-            return x < y;
-        });
-        const int64_t n_tasks = (int64_t)ord.size();
-        if (int rc = S.tasks.ensure((size_t)n_tasks * sizeof(Task))) return rc;
-        CK(cudaMemcpyAsync(S.order.p, ord.data(), (size_t)n_tasks * 4, cudaMemcpyHostToDevice, stream));
-        CK(cudaStreamSynchronize(stream));  // ord is pageable and reused per class
-        build_tasks_pairs_kernel<<<(unsigned)((n_tasks + 255) / 256), 256, 0, stream>>>(
-            S.tasks.as<Task>(), n_tasks, S.order.as<int32_t>(), S.pair_seq.as<int32_t>(), S.pair_ad.as<int32_t>(),
-            S.seq_off.as<int64_t>(), P.d_ad_off);
-        g_launches++;
-        CK(cudaGetLastError());
-        TaskSrc ts;
-        ts.tasks = S.tasks.as<Task>(); ts.n_tasks = n_tasks;
-        ts.cls_ad = nullptr; ts.n_cls_ad = 0; ts.n_adapters = n_adapters; ts.n_seqs = n_seqs;
-        ts.seq_off = S.seq_off.as<int64_t>(); ts.ad_off = P.d_ad_off; ts.seq_order = nullptr;
-        if (int rc = run_class_tasks(E, S, stream, c, m_max, ts, max_n, S.seq_codes.as<uint8_t>(), P.d_ad_codes,
-                                     P.sc, P.si, S.out.as<int32_t>(), status, counter)) return rc;
-    }
-    CK(cudaMemcpyAsync(out, S.out.p, (size_t)n_pairs * PB_REC * 4, cudaMemcpyDeviceToHost, stream));
-    return check_status(S, stream);
-    };
-    const int rc_pairs = run_pairs();
-    if (rc_pairs) {                         // nothing may still be reading the caller's buffers when we return
-        const std::string first_err = g_err;
-        cudaStreamSynchronize(E.st[0].stream);
-        g_err = first_err;
-    }
-    E.last_pending = false;                 // st[0] waited for an earlier call's queued work and is idle
-    return rc_pairs;
+        CK(cudaMemcpyAsync(out, S.out.p, (size_t)n_pairs * PB_REC * 4, cudaMemcpyDeviceToHost, stream));
+        return check_status(S, stream);
+    });
 }
 
 int batch_host_multi(const pb200_batch_t *batches, int n_batches, int ma, int mi, int go, int ge) {
@@ -1324,13 +1324,7 @@ int batch_host_multi(const pb200_batch_t *batches, int n_batches, int ma, int mi
                                    B.n_seqs * (int64_t)B.n_adapters, true)) return rc;
     }
     if (jobs.empty()) return 0;
-    Engine *Ep = nullptr;
-    if (int rc = get_engine(&Ep)) return rc;
-    Engine &E = *Ep;
-    std::lock_guard<std::mutex> lk(E.mu);
-    if (int rc = E.init()) return rc;
-    if (int rc = order_stages_after_last(E)) return rc;
-    return run_cross_jobs(E, jobs, ma, mi, go, ge);
+    return with_engine(CallOn::stages, nullptr, [&](Engine &E, cudaStream_t) { return run_cross_jobs(E, jobs, ma, mi, go, ge); });
 }
 
 // float("%f" % (100.0*c/l)) exactly as the reference chain produces it: std::to_string(double) = sprintf("%f")
@@ -1374,11 +1368,27 @@ std::shared_ptr<const std::vector<int32_t>> cached_threshold_table(double thr, i
     return t;
 }
 
+// a side without adapters: nothing aligns, nothing is trimmed, and the ranking has no pairs
+void fill_no_adapters(int32_t *trim, int32_t *top2, int64_t n_seqs) {
+    memset(trim, 0, (size_t)n_seqs * 4);
+    if (top2) for (int64_t s = 0; s < n_seqs; ++s) { int32_t *o = top2 + s * 6; o[0] = o[3] = -1; o[1] = o[4] = 0; o[2] = o[5] = 1; }
+}
+
+// The decision tables of decision job (or trim side) j: the end-trim threshold table and the score columns, on `stream`
+int upload_decision_tables(Engine &E, int j, cudaStream_t stream, double thr, int32_t cmin_len, const int32_t *score_cols,
+                           int32_t n_score_cols) {
+    const auto table = cached_threshold_table(thr, cmin_len);
+    if (int rc = E.dec_cmin[j].ensure((size_t)cmin_len * 4)) return rc;
+    if (int rc = E.dec_cols[j].ensure((size_t)std::max<int32_t>(n_score_cols, 1) * 4)) return rc;
+    CK(cudaMemcpyAsync(E.dec_cmin[j].p, table->data(), (size_t)cmin_len * 4, cudaMemcpyHostToDevice, stream));
+    if (n_score_cols > 0) CK(cudaMemcpyAsync(E.dec_cols[j].p, score_cols, (size_t)n_score_cols * 4, cudaMemcpyHostToDevice, stream));
+    return 0;
+}
+
 int batch_end_decisions(const pb200_end_batch_t *batches, int n_batches, int ma, int mi, int go, int ge) {
     if (n_batches < 0 || (n_batches > 0 && !batches)) return fail(PB200_ERR_ARG, "bad batch list");
     load_env_options();
     std::vector<CrossJob> jobs;
-    std::vector<std::shared_ptr<const std::vector<int32_t>>> tables;
     for (int b = 0; b < n_batches; ++b) {
         const pb200_end_batch_t &D = batches[b];
         const pb200_batch_t &B = D.batch;
@@ -1388,9 +1398,8 @@ int batch_end_decisions(const pb200_end_batch_t *batches, int n_batches, int ma,
         if (!(D.end_threshold >= 0.0)) return fail(PB200_ERR_ARG, "end_threshold must be >= 0 for the device decisions");
         for (int32_t k = 0; k < D.n_score_cols; ++k)
             if (D.score_cols[k] < 0 || D.score_cols[k] >= B.n_adapters) return fail(PB200_ERR_ARG, "score column out of range");
-        if (B.n_adapters == 0) {                 // no adapters: nothing aligns, nothing is trimmed
-            memset(D.trim, 0, (size_t)B.n_seqs * 4);
-            if (D.top2) for (int64_t s = 0; s < B.n_seqs; ++s) { int32_t *o = D.top2 + s * 6; o[0] = o[3] = -1; o[1] = o[4] = 0; o[2] = o[5] = 1; }
+        if (B.n_adapters == 0) {
+            fill_no_adapters(D.trim, D.top2, B.n_seqs);
             continue;
         }
         if (!B.seq_off || !B.ad_off) return fail(PB200_ERR_ARG, "NULL pointer");
@@ -1408,30 +1417,21 @@ int batch_end_decisions(const pb200_end_batch_t *batches, int n_batches, int ma,
         J.dec = &D;
         J.max_seq_len = D.end_size;
         J.cmin_len = (int32_t)(D.end_size + m_max + 2);
-        tables.push_back(cached_threshold_table(D.end_threshold, J.cmin_len));
         jobs.push_back(std::move(J));
     }
     if (jobs.empty()) return 0;
     if ((int)jobs.size() > Engine::MAX_DEC_JOBS) return fail(PB200_ERR_ARG, "too many decision batches in one call");
-    Engine *Ep = nullptr;
-    if (int rc = get_engine(&Ep)) return rc;
-    Engine &E = *Ep;
-    std::lock_guard<std::mutex> lk(E.mu);
-    if (int rc = E.init()) return rc;
-    if (int rc = order_stages_after_last(E)) return rc;
-    cudaStream_t s0 = E.st[0].stream;
-    for (size_t j = 0; j < jobs.size(); ++j) {
-        const pb200_end_batch_t &D = *jobs[j].dec;
-        if (int rc = E.dec_cmin[j].ensure((size_t)jobs[j].cmin_len * 4)) return rc;
-        if (int rc = E.dec_cols[j].ensure((size_t)std::max<int32_t>(D.n_score_cols, 1) * 4)) return rc;
-        CK(cudaMemcpyAsync(E.dec_cmin[j].p, tables[j]->data(), (size_t)jobs[j].cmin_len * 4, cudaMemcpyHostToDevice, s0));
-        if (D.n_score_cols > 0)
-            CK(cudaMemcpyAsync(E.dec_cols[j].p, D.score_cols, (size_t)D.n_score_cols * 4, cudaMemcpyHostToDevice, s0));
-        jobs[j].d_cmin = E.dec_cmin[j].as<int32_t>();
-        jobs[j].d_cols = E.dec_cols[j].as<int32_t>();
-    }
-    CK(cudaStreamSynchronize(s0));               // tables are in place before any stage's stream uses them
-    return run_cross_jobs(E, jobs, ma, mi, go, ge);
+    return with_engine(CallOn::stages, nullptr, [&](Engine &E, cudaStream_t s0) -> int {
+        for (size_t j = 0; j < jobs.size(); ++j) {
+            const pb200_end_batch_t &D = *jobs[j].dec;
+            if (int rc = upload_decision_tables(E, (int)j, s0, D.end_threshold, jobs[j].cmin_len, D.score_cols, D.n_score_cols))
+                return rc;
+            jobs[j].d_cmin = E.dec_cmin[j].as<int32_t>();
+            jobs[j].d_cols = E.dec_cols[j].as<int32_t>();
+        }
+        CK(cudaStreamSynchronize(s0));           // tables are in place before any stage's stream uses them
+        return run_cross_jobs(E, jobs, ma, mi, go, ge);
+    });
 }
 
 // Phase A on the device: every batch's records are max-reduced per adapter column (search_best_kernel) on the stage that made
@@ -1463,74 +1463,44 @@ int batch_search(const pb200_search_batch_t *batches, int n_batches, int ma, int
     for (int b = 0; b < n_batches; ++b)
         if (batches[b].batch.n_adapters > 0) std::fill(batches[b].best, batches[b].best + batches[b].batch.n_adapters, 0.0);
     if (jobs.empty()) return 0;
-    Engine *Ep = nullptr;
-    if (int rc = get_engine(&Ep)) return rc;
-    Engine &E = *Ep;
-    std::lock_guard<std::mutex> lk(E.mu);
-    if (int rc = E.init()) return rc;
-    if (int rc = order_stages_after_last(E)) return rc;
-    if (int rc = E.search_acc.ensure((size_t)NSTAGE * cols * 8)) return rc;
-    E.search_cols = cols;
-    for (int i = 0; i < NSTAGE; ++i)             // each slice is zeroed on the stream of the only stage that reduces into it
-        CK(cudaMemsetAsync(E.search_acc.as<unsigned long long>() + (size_t)i * cols, 0, (size_t)cols * 8, E.st[i].stream));
-    if (int rc = run_cross_jobs(E, jobs, ma, mi, go, ge)) return rc;
-    // run_cross_jobs drained every stage: the slices are final
-    std::vector<unsigned long long> keys((size_t)NSTAGE * cols);
-    CK(cudaMemcpyAsync(keys.data(), E.search_acc.p, keys.size() * 8, cudaMemcpyDeviceToHost, E.st[0].stream));
-    CK(cudaStreamSynchronize(E.st[0].stream));
-    for (size_t j = 0; j < jobs.size(); ++j) {
-        for (int32_t a = 0; a < jobs[j].n_adapters; ++a) {
-            unsigned long long k = 0;
-            for (int i = 0; i < NSTAGE; ++i) k = std::max(k, keys[(size_t)i * cols + jobs[j].search_col + a]);
-            double d;
-            memcpy(&d, &k, sizeof d);
-            bests[j][a] = printed_exact(d);
+    return with_engine(CallOn::stages, nullptr, [&](Engine &E, cudaStream_t s0) -> int {
+        if (int rc = E.search_acc.ensure((size_t)NSTAGE * cols * 8)) return rc;
+        E.search_cols = cols;
+        for (int i = 0; i < NSTAGE; ++i)         // each slice is zeroed on the stream of the only stage that reduces into it
+            CK(cudaMemsetAsync(E.search_acc.as<unsigned long long>() + (size_t)i * cols, 0, (size_t)cols * 8, E.st[i].stream));
+        if (int rc = run_cross_jobs(E, jobs, ma, mi, go, ge)) return rc;
+        // run_cross_jobs drained every stage: the slices are final
+        std::vector<unsigned long long> keys((size_t)NSTAGE * cols);
+        CK(cudaMemcpyAsync(keys.data(), E.search_acc.p, keys.size() * 8, cudaMemcpyDeviceToHost, s0));
+        CK(cudaStreamSynchronize(s0));
+        for (size_t j = 0; j < jobs.size(); ++j) {
+            for (int32_t a = 0; a < jobs[j].n_adapters; ++a) {
+                unsigned long long k = 0;
+                for (int i = 0; i < NSTAGE; ++i) k = std::max(k, keys[(size_t)i * cols + jobs[j].search_col + a]);
+                double d;
+                memcpy(&d, &k, sizeof d);
+                bests[j][a] = printed_exact(d);
+            }
         }
-    }
-    return 0;
+        return 0;
+    });
 }
 
-// longest sequence of a device-resident batch (S.misc must hold 64 bytes)
+// longest sequence of a device-resident batch, measured when *max_len < 0 (unknown); S.misc must hold 64 bytes
 int device_max_len(Stage &S, cudaStream_t stream, const int64_t *d_seq_off, int64_t n_seqs, int64_t *max_len) {
-    unsigned long long *d_max = reinterpret_cast<unsigned long long *>(S.misc.as<char>() + 32);
-    CK(cudaMemsetAsync(d_max, 0, 8, stream));
-    int64_t blocks = std::min<int64_t>((n_seqs + 255) / 256, 1024);
-    max_len_kernel<<<(unsigned)blocks, 256, 0, stream>>>(d_seq_off, n_seqs, d_max);
-    g_launches++;
-    CK(cudaGetLastError());
-    unsigned long long h = 0;
-    CK(cudaMemcpyAsync(&h, d_max, 8, cudaMemcpyDeviceToHost, stream));
-    CK(cudaStreamSynchronize(stream));
-    *max_len = (int64_t)h;
-    return 0;
-}
-
-int batch_device_queue(Engine &E, cudaStream_t stream, const uint8_t *d_seqs, const int64_t *d_seq_off, int64_t n_seqs,
-                       int64_t total_seq_bytes, int64_t max_seq_len, const uint8_t *adapters, const int32_t *ad_off,
-                       int32_t n_adapters, int ma, int mi, int go, int ge, int32_t *d_out);
-
-int batch_device(const uint8_t *d_seqs, const int64_t *d_seq_off, int64_t n_seqs, int64_t total_seq_bytes,
-                 int64_t max_seq_len, const uint8_t *adapters, const int32_t *ad_off, int32_t n_adapters, int ma, int mi,
-                 int go, int ge, int32_t *d_out, void *user_stream) {
-    if (n_seqs < 0 || n_adapters < 0 || total_seq_bytes < 0) return fail(PB200_ERR_ARG, "negative count");
-    if (n_seqs == 0 || n_adapters == 0) return 0;
-    if (!d_seq_off || !ad_off || !d_out) return fail(PB200_ERR_ARG, "NULL pointer");
-    Engine *Ep = nullptr;
-    if (int rc = get_engine(&Ep)) return rc;
-    Engine &E = *Ep;
-    std::lock_guard<std::mutex> lk(E.mu);
-    if (int rc = E.init()) return rc;
-    cudaStream_t stream = nullptr;
-    if (int rc = library_stream(E, user_stream, &stream)) return rc;
-    if (int rc = order_after_last(E, stream)) return rc;
-    // the work is queued on `stream` and the call returns without waiting for it: whatever happens below, the next call
-    // must wait for what was queued
-    const int rc = batch_device_queue(E, stream, d_seqs, d_seq_off, n_seqs, total_seq_bytes, max_seq_len, adapters, ad_off,
-                                      n_adapters, ma, mi, go, ge, d_out);
-    const std::string first_err = g_err;
-    const int rc_last = record_last(E, stream);
-    if (rc) { g_err = first_err; return rc; }
-    return rc_last;
+    if (*max_len < 0) {
+        unsigned long long *d_max = reinterpret_cast<unsigned long long *>(S.misc.as<char>() + 32);
+        CK(cudaMemsetAsync(d_max, 0, 8, stream));
+        int64_t blocks = std::min<int64_t>((n_seqs + 255) / 256, 1024);
+        max_len_kernel<<<(unsigned)blocks, 256, 0, stream>>>(d_seq_off, n_seqs, d_max);
+        g_launches++;
+        CK(cudaGetLastError());
+        unsigned long long h = 0;
+        CK(cudaMemcpyAsync(&h, d_max, 8, cudaMemcpyDeviceToHost, stream));
+        CK(cudaStreamSynchronize(stream));
+        *max_len = (int64_t)h;
+    }
+    return *max_len > 0x7fff0000ll ? fail(PB200_ERR_ARG, "sequence longer than 2^31") : 0;
 }
 
 int batch_device_queue(Engine &E, cudaStream_t stream, const uint8_t *d_seqs, const int64_t *d_seq_off, int64_t n_seqs,
@@ -1541,10 +1511,7 @@ int batch_device_queue(Engine &E, cudaStream_t stream, const uint8_t *d_seqs, co
     AdapterPlan P;
     if (int rc = plan_adapters(E, stream, adapters, ad_off, n_adapters, ma, mi, go, ge, P)) return rc;
     if (int rc = reset_misc(S, stream)) return rc;
-    if (max_seq_len < 0) {
-        if (int rc = device_max_len(S, stream, d_seq_off, n_seqs, &max_seq_len)) return rc;
-    }
-    if (max_seq_len > 0x7fff0000ll) return fail(PB200_ERR_ARG, "sequence longer than 2^31");
+    if (int rc = device_max_len(S, stream, d_seq_off, n_seqs, &max_seq_len)) return rc;
     const bool ascii = single_pass_ascii(P, max_seq_len);
     const uint8_t *seqs = d_seqs;
     if (!ascii) {
@@ -1575,6 +1542,23 @@ int batch_device_queue(Engine &E, cudaStream_t stream, const uint8_t *d_seqs, co
     return 0;
 }
 
+int batch_device(const uint8_t *d_seqs, const int64_t *d_seq_off, int64_t n_seqs, int64_t total_seq_bytes,
+                 int64_t max_seq_len, const uint8_t *adapters, const int32_t *ad_off, int32_t n_adapters, int ma, int mi,
+                 int go, int ge, int32_t *d_out, void *user_stream) {
+    if (n_seqs < 0 || n_adapters < 0 || total_seq_bytes < 0) return fail(PB200_ERR_ARG, "negative count");
+    if (n_seqs == 0 || n_adapters == 0) return 0;
+    if (!d_seq_off || !ad_off || !d_out) return fail(PB200_ERR_ARG, "NULL pointer");
+    return with_engine(CallOn::library, user_stream, [&](Engine &E, cudaStream_t stream) -> int {
+        // the work is queued on `stream` and the call returns without waiting for it: whatever happens below, the next call
+        // must wait for what was queued
+        const int rc = batch_device_queue(E, stream, d_seqs, d_seq_off, n_seqs, total_seq_bytes, max_seq_len, adapters, ad_off,
+                                          n_adapters, ma, mi, go, ge, d_out);
+        const std::string first_err = g_err;
+        const int rc_last = record_last(E, stream);
+        if (rc) { g_err = first_err; return rc; }
+        return rc_last;
+    });
+}
 
 // ---- middle-adapter scan (adapterMiddleScan, Phase C) ------------------------------------------------------------
 // Host-side checks that make the device loop exact and finite (include/porechop_b200.h): threshold > 0, adapters of A/C/G/T/U
@@ -1685,7 +1669,7 @@ int middle_rounds(Engine &E, Stage &S, cudaStream_t stream, const AdapterPlan &P
 // hits of every round of every segment -> n_hits / hits, sequence-major, each sequence's hits in round order
 int middle_emit(const std::vector<MiddleRound> &rounds, int64_t n_seqs, int32_t *n_hits, int32_t *hits, int64_t hits_cap,
                 int64_t *n_total) {
-    memset(n_hits, 0, (size_t)n_seqs * 4);
+    if (n_seqs > 0) memset(n_hits, 0, (size_t)n_seqs * 4);
     int64_t total = 0;
     for (const MiddleRound &R : rounds) {
         for (int32_t s : R.reads) n_hits[R.s0 + s]++;
@@ -1709,49 +1693,63 @@ int middle_table(Engine &E, cudaStream_t stream, double thr, int32_t cmin_len) {
     return 0;
 }
 
-int middle_check_outputs(int64_t n_seqs, int32_t n_adapters, const int32_t *n_hits, const int32_t *hits, int64_t hits_cap,
-                         const int64_t *n_total) {
+// Host reads: the buffer and the offsets checked, *max_len the longest read.
+int host_max_len(const uint8_t *seqs, const int64_t *seq_off, int64_t n_seqs, int64_t *max_len) {
+    if (int rc = validate_args(seqs, seq_off, n_seqs, nullptr, nullptr, 0, nullptr, nullptr, 0, true)) return rc;
+    *max_len = 0;
+    for (int64_t s = 0; s < n_seqs; ++s) {
+        const int64_t len = seq_off[s + 1] - seq_off[s];
+        if (len < 0) return fail(PB200_ERR_ARG, "sequence offsets not monotone");
+        *max_len = std::max(*max_len, len);
+    }
+    return *max_len > 0x7fff0000ll ? fail(PB200_ERR_ARG, "sequence longer than 2^31") : 0;
+}
+
+// Phase C of a segment whose reads are resident as codes (M.codes, M.off, longest M.max_len): round 0 over every read, chunk by
+// chunk, each chunk's DP followed by middle_decide_kernel from adapter 0; then the masking rounds.
+int middle_scan_resident(Engine &E, Stage &S, cudaStream_t stream, const AdapterPlan &P, MiddleSeg &M, int32_t n_adapters,
+                         const int32_t *h_ad_off, int64_t s0, std::vector<MiddleRound> &rounds) {
+    CK(cudaMemsetAsync(E.mid_ctr.p, 0, 16, stream));
+    const int64_t max_cnt = std::max<int64_t>(1, g_opt.device_chunk_tasks / n_adapters);
+    for (int64_t c0 = 0; c0 < M.n; c0 += max_cnt) {
+        const int64_t cnt = std::min(max_cnt, M.n - c0);
+        if (int rc = run_cross_chunk(E, S, stream, P, M.codes, M.off + c0, cnt, 0, M.max_len, n_adapters,
+                                     M.rec + (size_t)c0 * n_adapters * PB_REC, nullptr, 0, h_ad_off)) return rc;
+        if (int rc = launch_middle_decide(E, stream, M, n_adapters, nullptr, c0, cnt, M.active[0], S.misc.as<int>())) return rc;
+    }
+    return middle_rounds(E, S, stream, P, M, n_adapters, h_ad_off, s0, rounds);
+}
+
+// Entry checks of a middle scan (adapterMiddleScan*, and the middle adapters of adapterTrimReads*): the counts, the output
+// pointers, the adapters and the scan's preconditions; *cmin_len: the length of its threshold table.  The reads are the
+// caller's to check.
+int middle_entry_checks(int64_t n_seqs, const uint8_t *adapters, const int32_t *ad_off, int32_t n_adapters, int ma, int mi,
+                        int go, int ge, double thr, const int32_t *n_hits, const int32_t *hits, int64_t hits_cap,
+                        const int64_t *n_total, int32_t *cmin_len) {
     if (n_seqs < 0 || n_adapters < 0 || hits_cap < 0) return fail(PB200_ERR_ARG, "negative count");
-    if (!n_total || (n_seqs > 0 && !n_hits) || (hits_cap > 0 && !hits)) return fail(PB200_ERR_ARG, "NULL pointer");
-    return 0;
+    if (!n_total || (n_seqs > 0 && !n_hits) || (hits_cap > 0 && !hits) || (n_adapters > 0 && !ad_off))
+        return fail(PB200_ERR_ARG, "NULL pointer");
+    *cmin_len = 0;
+    if (n_adapters == 0) return thr > 0.0 ? 0 : fail(PB200_ERR_ARG, "middle_threshold must be > 0 for the device middle scan");
+    if (int rc = validate_args(nullptr, nullptr, 0, adapters, ad_off, n_adapters, nullptr, nullptr, 0, true)) return rc;
+    return middle_preconditions(adapters, ad_off, n_adapters, ma, mi, go, ge, thr, cmin_len);
 }
 
 int middle_host(const uint8_t *seqs, const int64_t *seq_off, int64_t n_seqs, const uint8_t *adapters, const int32_t *ad_off,
                 int32_t n_adapters, int ma, int mi, int go, int ge, double thr, int32_t *n_hits, int32_t *hits,
                 int64_t hits_cap, int64_t *n_total) {
-    if (int rc = middle_check_outputs(n_seqs, n_adapters, n_hits, hits, hits_cap, n_total)) return rc;
-    if (n_seqs > 0 && (!seq_off || (n_adapters > 0 && !ad_off))) return fail(PB200_ERR_ARG, "NULL pointer");
     load_env_options();
     int32_t cmin_len = 0;
-    if (n_adapters > 0) {
-        if (int rc = validate_args(seqs, seq_off, n_seqs, adapters, ad_off, n_adapters, nullptr, nullptr, 0, true)) return rc;
-        if (int rc = middle_preconditions(adapters, ad_off, n_adapters, ma, mi, go, ge, thr, &cmin_len)) return rc;
-    } else if (!(thr > 0.0)) {
-        return fail(PB200_ERR_ARG, "middle_threshold must be > 0 for the device middle scan");
-    }
-    if (n_seqs == 0 || n_adapters == 0) {
-        if (n_seqs > 0) memset(n_hits, 0, (size_t)n_seqs * 4);
-        *n_total = 0;
-        return 0;
-    }
+    if (int rc = middle_entry_checks(n_seqs, adapters, ad_off, n_adapters, ma, mi, go, ge, thr, n_hits, hits, hits_cap, n_total,
+                                     &cmin_len)) return rc;
+    if (n_seqs > 0 && !seq_off) return fail(PB200_ERR_ARG, "NULL pointer");
+    if (n_seqs == 0 || n_adapters == 0) return middle_emit({}, n_seqs, n_hits, hits, hits_cap, n_total);
     int64_t max_len = 0;
-    for (int64_t s = 0; s < n_seqs; ++s) {
-        const int64_t len = seq_off[s + 1] - seq_off[s];
-        if (len < 0) return fail(PB200_ERR_ARG, "sequence offsets not monotone");
-        max_len = std::max(max_len, len);
-    }
-    if (max_len > 0x7fff0000ll) return fail(PB200_ERR_ARG, "sequence longer than 2^31");
-    Engine *Ep = nullptr;
-    if (int rc = get_engine(&Ep)) return rc;
-    Engine &E = *Ep;
-    std::lock_guard<std::mutex> lk(E.mu);
-    if (int rc = E.init()) return rc;
-    if (int rc = order_stages_after_last(E)) return rc;
-    NvtxRange submit_range("pb200:submit_middle");
-    Stage &S = E.st[0];
-    cudaStream_t stream = S.stream;
+    if (int rc = host_max_len(seqs, seq_off, n_seqs, &max_len)) return rc;
     std::vector<MiddleRound> rounds;
-    auto run = [&]() -> int {
+    const int rc = sync_call(CallOn::stages, nullptr, [&](Engine &E, cudaStream_t stream) -> int {
+        NvtxRange submit_range("pb200:submit_middle");
+        Stage &S = E.st[0];
         if (int rc = middle_table(E, stream, thr, cmin_len)) return rc;
         for (int64_t a = 0; a < n_seqs;) {
             const int64_t b = middle_segment_end(E, a, n_seqs, n_adapters, seq_off);
@@ -1773,14 +1771,7 @@ int middle_host(const uint8_t *seqs, const int64_t *seq_off, int64_t n_seqs, con
             a = b;
         }
         return 0;
-    };
-    const int rc = run();
-    if (rc) {                             // nothing may still be running when we return
-        const std::string first_err = g_err;
-        cudaStreamSynchronize(stream);
-        g_err = first_err;
-    }
-    E.last_pending = false;               // the streams waited for an earlier call's queued work and are idle
+    });
     if (rc) return rc;
     return middle_emit(rounds, n_seqs, n_hits, hits, hits_cap, n_total);
 }
@@ -1789,34 +1780,17 @@ int middle_device(const uint8_t *d_seqs, const int64_t *d_seq_off, int64_t n_seq
                   int64_t max_seq_len, const uint8_t *adapters, const int32_t *ad_off, int32_t n_adapters, int ma, int mi,
                   int go, int ge, double thr, int32_t *n_hits, int32_t *hits, int64_t hits_cap, int64_t *n_total,
                   void *user_stream) {
-    if (int rc = middle_check_outputs(n_seqs, n_adapters, n_hits, hits, hits_cap, n_total)) return rc;
     if (total_seq_bytes < 0) return fail(PB200_ERR_ARG, "negative count");
-    if (n_seqs > 0 && (!d_seq_off || (n_adapters > 0 && !ad_off))) return fail(PB200_ERR_ARG, "NULL pointer");
     load_env_options();
     int32_t cmin_len = 0;
-    if (n_adapters > 0) {
-        if (int rc = validate_args(nullptr, nullptr, 0, adapters, ad_off, n_adapters, nullptr, nullptr, 0, true)) return rc;
-        if (int rc = middle_preconditions(adapters, ad_off, n_adapters, ma, mi, go, ge, thr, &cmin_len)) return rc;
-    } else if (!(thr > 0.0)) {
-        return fail(PB200_ERR_ARG, "middle_threshold must be > 0 for the device middle scan");
-    }
-    if (n_seqs == 0 || n_adapters == 0) {
-        if (n_seqs > 0) memset(n_hits, 0, (size_t)n_seqs * 4);
-        *n_total = 0;
-        return 0;
-    }
-    Engine *Ep = nullptr;
-    if (int rc = get_engine(&Ep)) return rc;
-    Engine &E = *Ep;
-    std::lock_guard<std::mutex> lk(E.mu);
-    if (int rc = E.init()) return rc;
-    Stage &S = E.st[0];
-    cudaStream_t stream = nullptr;
-    if (int rc = library_stream(E, user_stream, &stream)) return rc;
-    if (int rc = order_after_last(E, stream)) return rc;
-    NvtxRange submit_range("pb200:submit_middle");
+    if (int rc = middle_entry_checks(n_seqs, adapters, ad_off, n_adapters, ma, mi, go, ge, thr, n_hits, hits, hits_cap, n_total,
+                                     &cmin_len)) return rc;
+    if (n_seqs > 0 && !d_seq_off) return fail(PB200_ERR_ARG, "NULL pointer");
+    if (n_seqs == 0 || n_adapters == 0) return middle_emit({}, n_seqs, n_hits, hits, hits_cap, n_total);
     std::vector<MiddleRound> rounds;
-    auto run = [&]() -> int {
+    const int rc = sync_call(CallOn::library, user_stream, [&](Engine &E, cudaStream_t stream) -> int {
+        NvtxRange submit_range("pb200:submit_middle");
+        Stage &S = E.st[0];
         if (!S.misc.p) {
             if (int rc = S.misc.ensure(64)) return rc;
             CK(cudaMemsetAsync(S.misc.p, 0, 64, stream));
@@ -1824,10 +1798,7 @@ int middle_device(const uint8_t *d_seqs, const int64_t *d_seq_off, int64_t n_seq
         if (int rc = check_status(S, stream)) return rc;     // a deferred error of an earlier device-resident call
         AdapterPlan P;
         if (int rc = plan_adapters(E, stream, adapters, ad_off, n_adapters, ma, mi, go, ge, P)) return rc;
-        if (max_seq_len < 0) {
-            if (int rc = device_max_len(S, stream, d_seq_off, n_seqs, &max_seq_len)) return rc;
-        }
-        if (max_seq_len > 0x7fff0000ll) return fail(PB200_ERR_ARG, "sequence longer than 2^31");
+        if (int rc = device_max_len(S, stream, d_seq_off, n_seqs, &max_seq_len)) return rc;
         if (int rc = middle_table(E, stream, thr, cmin_len)) return rc;
         // the library's encoded copy of the caller's sequences is what the rounds mask
         if (int rc = E.mid_codes.ensure((size_t)total_seq_bytes + 16)) return rc;
@@ -1840,27 +1811,11 @@ int middle_device(const uint8_t *d_seqs, const int64_t *d_seq_off, int64_t n_seq
             M.off = const_cast<int64_t *>(d_seq_off + a);          // read only: offsets are written by the host-buffer path only
             M.cmin_len = cmin_len;
             M.max_len = max_seq_len;
-            CK(cudaMemsetAsync(E.mid_ctr.p, 0, 16, stream));
-            const int64_t max_cnt = std::max<int64_t>(1, g_opt.device_chunk_tasks / n_adapters);
-            for (int64_t c0 = 0; c0 < b - a; c0 += max_cnt) {           // round 0: every read, from adapter 0
-                const int64_t cnt = std::min(max_cnt, b - a - c0);
-                if (int rc = run_cross_chunk(E, S, stream, P, M.codes, M.off + c0, cnt, 0, max_seq_len, n_adapters,
-                                             M.rec + (size_t)c0 * n_adapters * PB_REC, nullptr, 0, ad_off)) return rc;
-                if (int rc = launch_middle_decide(E, stream, M, n_adapters, nullptr, c0, cnt, M.active[0], S.misc.as<int>()))
-                    return rc;
-            }
-            if (int rc = middle_rounds(E, S, stream, P, M, n_adapters, ad_off, a, rounds)) return rc;
+            if (int rc = middle_scan_resident(E, S, stream, P, M, n_adapters, ad_off, a, rounds)) return rc;
             a = b;
         }
         return 0;
-    };
-    const int rc = run();
-    if (rc) {
-        const std::string first_err = g_err;
-        cudaStreamSynchronize(stream);
-        g_err = first_err;
-    }
-    E.last_pending = false;
+    });
     if (rc) return rc;
     return middle_emit(rounds, n_seqs, n_hits, hits, hits_cap, n_total);
 }
@@ -2137,13 +2092,17 @@ int demux_finalize(Engine &E, Stage &S, cudaStream_t stream, const pb200_split_a
     return 0;
 }
 
-// device: seqs / seq_off are device pointers (adapterTrimReadsDevice), else host buffers uploaded segment by segment.
-// X: the output stage of adapterTrimSplitReadsDevice (device reads only), or nullptr.  Dm: the demux stage of
-// adapterDemuxReadsDevice (with X), or nullptr.
-int trim_reads(const uint8_t *seqs, const int64_t *seq_off, int64_t n_seqs, bool device, int64_t total_seq_bytes,
-               int64_t max_seq_len, const pb200_trim_args_t *A, int ma, int mi, int go, int ge, void *user_stream,
-               const pb200_split_args_t *X = nullptr, const pb200_demux_args_t *Dm = nullptr) {
-    // ---- preconditions: nothing below touches the device before they all hold ----
+// What the preconditions of a whole-read call establish before anything touches the device: the threshold-table lengths of
+// both sides and of the middle scan, the longest read (-1: measured on the device) and the demux stage's score table.
+struct TrimPlan {
+    int32_t cmin_len[2] = {0, 0}, mid_cmin_len = 0;
+    int64_t max_len = -1;
+    DemuxStage dstage;
+};
+
+int trim_plan(const uint8_t *seqs, const int64_t *seq_off, int64_t n_seqs, bool device, int64_t total_seq_bytes,
+              int64_t max_seq_len, const pb200_trim_args_t *A, int ma, int mi, int go, int ge, const pb200_split_args_t *X,
+              const pb200_demux_args_t *Dm, TrimPlan &TP) {
     if (!A) return fail(PB200_ERR_ARG, "NULL pointer");
     if (n_seqs < 0 || total_seq_bytes < 0) return fail(PB200_ERR_ARG, "negative count");
     if (A->end_size < 1) return fail(PB200_ERR_ARG, "end_size must be >= 1");
@@ -2151,30 +2110,18 @@ int trim_reads(const uint8_t *seqs, const int64_t *seq_off, int64_t n_seqs, bool
     load_env_options();
     const SchemeInfo si = scheme_info(ma, mi, go, ge);
     const pb200_trim_side_t *side[2] = {&A->start, &A->end};
-    int32_t cmin_len[2] = {0, 0}, mid_cmin_len = 0;
     for (int k = 0; k < 2; ++k)
-        if (int rc = trim_side_check(*side[k], n_seqs, A->end_size, si, &cmin_len[k], Dm != nullptr)) return rc;
+        if (int rc = trim_side_check(*side[k], n_seqs, A->end_size, si, &TP.cmin_len[k], Dm != nullptr)) return rc;
     const int32_t n_mid = A->n_mid_adapters;
     if (n_mid < 0) return fail(PB200_ERR_ARG, "negative count");
     if (n_mid > 0) {
-        if (int rc = middle_check_outputs(n_seqs, n_mid, A->n_hits, A->hits, A->hits_cap, A->n_total)) return rc;
-        if (!A->mid_ad_off) return fail(PB200_ERR_ARG, "NULL pointer");
-        if (int rc = validate_args(nullptr, nullptr, 0, A->mid_adapters, A->mid_ad_off, n_mid, nullptr, nullptr, 0, true)) return rc;
-        if (int rc = middle_preconditions(A->mid_adapters, A->mid_ad_off, n_mid, ma, mi, go, ge, A->middle_threshold, &mid_cmin_len))
-            return rc;
+        if (int rc = middle_entry_checks(n_seqs, A->mid_adapters, A->mid_ad_off, n_mid, ma, mi, go, ge, A->middle_threshold,
+                                         A->n_hits, A->hits, A->hits_cap, A->n_total, &TP.mid_cmin_len)) return rc;
     }
     if (n_seqs > 0 && !seq_off) return fail(PB200_ERR_ARG, "NULL pointer");
-    int64_t max_len = max_seq_len;
-    if (!device && n_seqs > 0) {
-        if (int rc = validate_args(seqs, seq_off, n_seqs, nullptr, nullptr, 0, nullptr, nullptr, 0, true)) return rc;
-        max_len = 0;
-        for (int64_t s = 0; s < n_seqs; ++s) {
-            const int64_t len = seq_off[s + 1] - seq_off[s];
-            if (len < 0) return fail(PB200_ERR_ARG, "sequence offsets not monotone");
-            max_len = std::max(max_len, len);
-        }
-    }
-    if (max_len > 0x7fff0000ll) return fail(PB200_ERR_ARG, "sequence longer than 2^31");
+    TP.max_len = max_seq_len;
+    if (!device && n_seqs > 0) { if (int rc = host_max_len(seqs, seq_off, n_seqs, &TP.max_len)) return rc; }
+    if (TP.max_len > 0x7fff0000ll) return fail(PB200_ERR_ARG, "sequence longer than 2^31");
     if (X) {
         if (!device) return fail(PB200_ERR_ARG, "the output stage takes device reads only");
         if (X->parts_cap < 0) return fail(PB200_ERR_ARG, "negative count");
@@ -2185,7 +2132,6 @@ int trim_reads(const uint8_t *seqs, const int64_t *seq_off, int64_t n_seqs, bool
                                                                   (total_seq_bytes > 0 && !X->d_out_seq)))))
             return fail(PB200_ERR_ARG, "NULL pointer");
     }
-    DemuxStage dstage;
     if (Dm) {
         if (!X) return fail(PB200_ERR_ARG, "the demux stage needs the output stage");
         if (!Dm->read_bin || !Dm->bin_parts) return fail(PB200_ERR_ARG, "NULL pointer");
@@ -2205,232 +2151,250 @@ int trim_reads(const uint8_t *seqs, const int64_t *seq_off, int64_t n_seqs, bool
                 seen[(size_t)map[j]] = 1;
             }
             // the score table covers every (match_ad, len_ad) of the side: match_ad <= its longest adapter, len_ad < cmin_len
-            dstage.tab_c = std::max(dstage.tab_c, cmin_len[k] - A->end_size - 1);
-            dstage.tab_l = std::max(dstage.tab_l, cmin_len[k]);
+            TP.dstage.tab_c = std::max(TP.dstage.tab_c, TP.cmin_len[k] - A->end_size - 1);
+            TP.dstage.tab_l = std::max(TP.dstage.tab_l, TP.cmin_len[k]);
         }
-        memset(Dm->bin_parts, 0, (size_t)(Dm->n_bins + 2) * 8);
     }
-    if (A->n_hits && n_seqs > 0) memset(A->n_hits, 0, (size_t)n_seqs * 4);
-    if (A->n_total) *A->n_total = 0;
-    for (int k = 0; k < 2; ++k) {         // a side without adapters: nothing aligns, nothing is trimmed
-        const pb200_trim_side_t &T = *side[k];
-        if (T.n_adapters > 0 || n_seqs == 0) continue;
-        memset(T.trim, 0, (size_t)n_seqs * 4);
-        if (T.top2) for (int64_t s = 0; s < n_seqs; ++s) { int32_t *o = T.top2 + s * 6; o[0] = o[3] = -1; o[1] = o[4] = 0; o[2] = o[5] = 1; }
-    }
-    // without adapters nothing is trimmed or split; the output stage still writes every non-empty read ("No adapters found")
-    if (n_seqs == 0 || (!X && A->start.n_adapters == 0 && A->end.n_adapters == 0 && n_mid == 0)) return 0;
+    return 0;
+}
 
-    Engine *Ep = nullptr;
-    if (int rc = get_engine(&Ep)) return rc;
-    Engine &E = *Ep;
-    std::lock_guard<std::mutex> lk(E.mu);
-    if (int rc = E.init()) return rc;
-    Stage &S = E.st[0];
-    cudaStream_t stream = S.stream;
-    if (device) { if (int rc = library_stream(E, user_stream, &stream)) return rc; }
-    if (int rc = order_after_last(E, stream)) return rc;
-    NvtxRange submit_range(Dm ? "pb200:submit_demux" : X ? "pb200:submit_trim_split" : "pb200:submit_trim");
-    std::vector<MiddleRound> rounds;
-    SplitTotals totals;
-    auto run = [&]() -> int {
+// The device work of a whole-read call on its stream, stage by stage.  device: seqs / seq_off are device pointers
+// (adapterTrimReadsDevice), else host buffers uploaded segment by segment.  X: the output stage of adapterTrimSplitReadsDevice
+// (device reads only), or nullptr.  Dm: the demux stage of adapterDemuxReadsDevice (with X), or nullptr.
+struct TrimCall {
+    Engine &E; Stage &S; cudaStream_t stream;
+    const uint8_t *seqs; const int64_t *seq_off; int64_t n_seqs; bool device; int64_t total_seq_bytes;
+    const pb200_trim_args_t &A; const pb200_split_args_t *X; const pb200_demux_args_t *Dm;
+    TrimPlan &TP;
+    std::vector<MiddleRound> &rounds;
+    SplitTotals &totals;
+    AdapterPlan P[2], PM;                 // the adapter plans of both sides and of the middle scan
+    int64_t wl_max = 0;                   // the longest end window
+
+    const pb200_trim_side_t &side(int k) const { return k ? A.end : A.start; }
+
+    int run(int ma, int mi, int go, int ge) {
         if (int rc = reset_misc(S, stream)) return rc;
         if (int rc = check_status(S, stream)) return rc;     // a deferred error of an earlier device-resident call
-        AdapterPlan P[2], PM;
+        if (int rc = upload_tables(ma, mi, go, ge)) return rc;
+        if (int rc = device_max_len(S, stream, seq_off, n_seqs, &TP.max_len)) return rc;
+        wl_max = std::min<int64_t>(A.end_size, TP.max_len);
+        if (device && A.n_mid_adapters > 0) { if (int rc = E.mid_codes.ensure((size_t)total_seq_bytes + 16)) return rc; }
+        for (int64_t a = 0; a < n_seqs;) {
+            const int64_t b = trim_segment_end(E, a, n_seqs, A.n_mid_adapters, wl_max, device ? nullptr : seq_off, X != nullptr,
+                                               Dm != nullptr);
+            if (int rc = segment(a, b - a)) return rc;
+            a = b;
+        }
+        if (Dm) { if (int rc = demux_finalize(E, S, stream, *X, *Dm, seqs, n_seqs, totals)) return rc; }
+        if (X) CK(cudaStreamSynchronize(stream));      // the device outputs are written when the call returns
+        return 0;
+    }
+
+    // Reads [a, a + n): end windows, Phase B of both sides, the barcode call; then, with middle adapters or an output stage,
+    // the trimmed ranges, Phase C and the output records.
+    int segment(int64_t a, int64_t n) {
+        const uint8_t *reads = nullptr;
+        const int64_t *off = nullptr;
+        if (int rc = segment_reads(a, n, reads, off)) return rc;
+        int64_t win_total = -1;
+        for (int k = 0; k < 2; ++k)
+            if (int rc = end_side(k, a, n, win_total)) return rc;
+        if (Dm) { if (int rc = barcode_call(a, n)) return rc; }
+        const int32_t n_mid = A.n_mid_adapters;
+        if (n_mid == 0) {
+            if (int rc = check_status(S, stream)) return rc;
+            if (!X) return 0;
+        }
+        MiddleSeg M;
+        if (n_mid > 0) {
+            if (int rc = middle_segment_buffers(E, n, n_mid, device ? 0 : (size_t)(seq_off[a + n] - seq_off[a]), M)) return rc;
+        }
+        if (int rc = trimmed_ranges(off, n)) return rc;
+        const size_t r0 = rounds.size();
+        if (n_mid > 0) { if (int rc = middle_scan(reads, off, a, M)) return rc; }
+        if (!X) return 0;
+        return split_segment(E, stream, *X, reads, off, a, n, E.trim_first.as<int64_t>(), E.mid_off.as<int64_t>(), rounds, r0,
+                             totals, Dm ? &TP.dstage : nullptr);
+    }
+
+    // Per call: both sides' adapter plans and decision tables; the demux stage's bin of each score column, score table and
+    // per-read bins; the middle scan's plan and threshold table.
+    int upload_tables(int ma, int mi, int go, int ge) {
         for (int k = 0; k < 2; ++k) {
-            const pb200_trim_side_t &T = *side[k];
+            const pb200_trim_side_t &T = side(k);
             if (T.n_adapters == 0) continue;
             if (int rc = plan_adapters(E, stream, T.adapters, T.ad_off, T.n_adapters, ma, mi, go, ge, P[k])) return rc;
-            const auto table = cached_threshold_table(A->end_threshold, cmin_len[k]);
-            if (int rc = E.dec_cmin[k].ensure((size_t)cmin_len[k] * 4)) return rc;
-            if (int rc = E.dec_cols[k].ensure((size_t)std::max<int32_t>(T.n_score_cols, 1) * 4)) return rc;
-            CK(cudaMemcpyAsync(E.dec_cmin[k].p, table->data(), (size_t)cmin_len[k] * 4, cudaMemcpyHostToDevice, stream));
-            if (T.n_score_cols > 0)
-                CK(cudaMemcpyAsync(E.dec_cols[k].p, T.score_cols, (size_t)T.n_score_cols * 4, cudaMemcpyHostToDevice, stream));
+            if (int rc = upload_decision_tables(E, k, stream, A.end_threshold, TP.cmin_len[k], T.score_cols, T.n_score_cols))
+                return rc;
         }
         if (Dm) {                             // the call rule's inputs: bin of each score column, score table; a bin per read
             for (int k = 0; k < 2; ++k) {
-                const int32_t n_cols = side[k]->n_score_cols;
+                const int32_t n_cols = side(k).n_score_cols;
                 if (n_cols == 0) continue;
                 if (int rc = E.demux_map[k].ensure((size_t)n_cols * 4)) return rc;
                 CK(cudaMemcpyAsync(E.demux_map[k].p, k ? Dm->end_bin : Dm->start_bin, (size_t)n_cols * 4, cudaMemcpyHostToDevice,
                                    stream));
             }
-            if (dstage.tab_c > 0) {
-                const auto tab = cached_score_table(dstage.tab_c, dstage.tab_l);
+            if (TP.dstage.tab_c > 0) {
+                const auto tab = cached_score_table(TP.dstage.tab_c, TP.dstage.tab_l);
                 if (int rc = E.demux_tab.ensure(tab->size() * 8)) return rc;
                 CK(cudaMemcpyAsync(E.demux_tab.p, tab->data(), tab->size() * 8, cudaMemcpyHostToDevice, stream));
             }
             if (int rc = E.demux_bin.ensure((size_t)n_seqs * 4 + 16)) return rc;
         }
-        if (n_mid > 0) {
-            if (int rc = plan_adapters(E, stream, A->mid_adapters, A->mid_ad_off, n_mid, ma, mi, go, ge, PM)) return rc;
-            if (int rc = middle_table(E, stream, A->middle_threshold, mid_cmin_len)) return rc;   // (synchronises the stream)
+        if (A.n_mid_adapters > 0) {
+            if (int rc = plan_adapters(E, stream, A.mid_adapters, A.mid_ad_off, A.n_mid_adapters, ma, mi, go, ge, PM)) return rc;
+            if (int rc = middle_table(E, stream, A.middle_threshold, TP.mid_cmin_len)) return rc;   // (synchronises the stream)
         }
-        if (max_len < 0) {
-            if (int rc = device_max_len(S, stream, seq_off, n_seqs, &max_len)) return rc;
-            if (max_len > 0x7fff0000ll) return fail(PB200_ERR_ARG, "sequence longer than 2^31");
-        }
-        const int64_t wl_max = std::min<int64_t>(A->end_size, max_len);
-        if (device && n_mid > 0) {
-            if (int rc = E.mid_codes.ensure((size_t)total_seq_bytes + 16)) return rc;
-        }
-        for (int64_t a = 0; a < n_seqs;) {
-            const int64_t b = trim_segment_end(E, a, n_seqs, n_mid, wl_max, device ? nullptr : seq_off, X != nullptr, Dm != nullptr);
-            const int64_t n = b - a;
-            // the segment's reads: ASCII at reads[off[s] .. off[s+1])
-            const uint8_t *reads = seqs;
-            const int64_t *off = seq_off + a;
-            int64_t bytes = 0;
-            if (!device) {                   // the only upload of read bytes
-                bytes = seq_off[b] - seq_off[a];
-                if (int rc = E.trim_reads.ensure((size_t)bytes + 16)) return rc;
-                if (int rc = E.trim_off.ensure((size_t)(n + 1) * 8)) return rc;
-                if (bytes) CK(cudaMemcpyAsync(E.trim_reads.p, seqs + seq_off[a], (size_t)bytes, cudaMemcpyHostToDevice, stream));
-                CK(cudaMemcpyAsync(E.trim_off.p, seq_off + a, (size_t)(n + 1) * 8, cudaMemcpyHostToDevice, stream));
-                rebase_kernel<<<(unsigned)((n + 1 + 255) / 256), 256, 0, stream>>>(E.trim_off.as<int64_t>(), n + 1, seq_off[a]);
-                g_launches++;
-                reads = E.trim_reads.as<uint8_t>();
-                off = E.trim_off.as<int64_t>();
-            }
-            const int64_t warp_blocks = std::max<int64_t>(1, std::min<int64_t>((n + 3) / 4, (int64_t)E.sm_count * 16));
-            // ---- end windows: lengths, offsets (shared by both sides), the cut ----
-            const size_t win_bytes = (size_t)n * (size_t)wl_max;
-            if (int rc = E.trim_win_off.ensure((size_t)(n + 1) * 8)) return rc;
-            if (int rc = E.trim_win[0].ensure(win_bytes + 16)) return rc;
-            if (int rc = E.trim_win[1].ensure(win_bytes + 16)) return rc;
-            int64_t *win_off = E.trim_win_off.as<int64_t>();
-            window_len_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(off, n, (int64_t)A->end_size, win_off);
-            g_launches++;
-            if (int rc = scan_offsets(E, stream, win_off, n)) return rc;
-            cut_windows_kernel<<<(unsigned)warp_blocks, 128, 0, stream>>>(reads, off, static_cast<const int64_t *>(win_off), n,
-                                                                         E.trim_win[0].as<uint8_t>(), E.trim_win[1].as<uint8_t>());
-            g_launches++;
-            CK(cudaGetLastError());
-            // ---- Phase B, side by side: DP chunks, then decide_kernel into the segment-wide trims ----
-            int64_t win_total = -1;
-            for (int k = 0; k < 2; ++k) {
-                const pb200_trim_side_t &T = *side[k];
-                if (int rc = E.trim_d[k].ensure((size_t)n * 4 + 16)) return rc;
-                if (T.n_adapters == 0) {
-                    CK(cudaMemsetAsync(E.trim_d[k].p, 0, (size_t)n * 4, stream));
-                    continue;
-                }
-                const bool ascii = single_pass_ascii(P[k], wl_max);
-                const uint8_t *w = E.trim_win[k].as<uint8_t>();
-                if (!ascii) {                // two-pass windows: encode first, as batch_device_queue does
-                    if (win_total < 0) {
-                        CK(cudaMemcpyAsync(&win_total, win_off + n, 8, cudaMemcpyDeviceToHost, stream));
-                        CK(cudaStreamSynchronize(stream));
-                    }
-                    if (int rc = S.seq_codes.ensure((size_t)win_total + 16)) return rc;
-                    if (int rc = launch_encode(stream, w, S.seq_codes.as<uint8_t>(), win_total, E.sm_count)) return rc;
-                    w = S.seq_codes.as<uint8_t>();
-                }
-                pb200_end_batch_t D;
-                memset(&D, 0, sizeof D);
-                D.is_start = k == 0 ? 1 : 0; D.end_size = A->end_size; D.extra_trim_size = A->extra_trim_size;
-                D.min_trim_size = A->min_trim_size; D.end_threshold = A->end_threshold;
-                D.score_cols = T.score_cols; D.n_score_cols = T.n_score_cols;
-                D.trim = T.trim; D.score_pairs = T.score_pairs; D.top2 = T.top2;
-                const int64_t max_cnt = std::max<int64_t>(1, g_opt.device_chunk_tasks / T.n_adapters);
-                int32_t *top2 = nullptr;     // demux: the segment's ranking stays on the device for barcode_call_kernel
-                if (Dm && T.n_score_cols > 0) {
-                    if (int rc = E.demux_top2[k].ensure((size_t)n * 6 * 4 + 16)) return rc;
-                    top2 = E.demux_top2[k].as<int32_t>();
-                }
-                for (int64_t c0 = 0; c0 < n; c0 += max_cnt) {
-                    const int64_t cnt = std::min(max_cnt, n - c0);
-                    if (int rc = S.out.ensure((size_t)cnt * T.n_adapters * PB_REC * 4)) return rc;
-                    if (int rc = run_cross_chunk(E, S, stream, P[k], w, win_off + c0, cnt, 0, wl_max, T.n_adapters,
-                                                 S.out.as<int32_t>(), nullptr, 0, T.ad_off, nullptr, ascii)) return rc;
-                    if (int rc = launch_decide(E, S, stream, D, S.out.as<int32_t>(), cnt, T.n_adapters, E.dec_cmin[k].as<int32_t>(),
-                                               cmin_len[k], E.dec_cols[k].as<int32_t>(), E.trim_d[k].as<int32_t>() + c0, a + c0,
-                                               top2 ? top2 + c0 * 6 : nullptr))
-                        return rc;
-                }
-            }
-            if (Dm) {                        // ---- the barcode call of every read of the segment ----
-                const int32_t *t[2] = {nullptr, nullptr};
-                for (int k = 0; k < 2; ++k) if (side[k]->n_score_cols > 0) t[k] = E.demux_top2[k].as<int32_t>();
-                barcode_call_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(
-                    t[0], t[1], static_cast<const int32_t *>(E.demux_map[0].as<int32_t>()),
-                    static_cast<const int32_t *>(E.demux_map[1].as<int32_t>()), static_cast<const double *>(E.demux_tab.as<double>()),
-                    dstage.tab_c, dstage.tab_l, n, Dm->n_bins, Dm->barcode_threshold, Dm->barcode_diff, Dm->require_two_barcodes,
-                    Dm->d_albacore ? Dm->d_albacore + a : nullptr, E.demux_bin.as<int32_t>() + a, S.misc.as<int>());
-                g_launches++;
-                CK(cudaGetLastError());
-            }
-            if (n_mid == 0) {
-                if (int rc = check_status(S, stream)) return rc;
-                if (X) {                     // the trimmed ranges the middle scan would have made, then the output stage
-                    if (int rc = E.trim_first.ensure((size_t)n * 8 + 16)) return rc;
-                    if (int rc = E.mid_off.ensure((size_t)(n + 1) * 8)) return rc;
-                    int64_t *toff = E.mid_off.as<int64_t>();
-                    trimmed_range_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(
-                        off, static_cast<const int32_t *>(E.trim_d[0].as<int32_t>()), static_cast<const int32_t *>(E.trim_d[1].as<int32_t>()),
-                        n, E.trim_first.as<int64_t>(), toff);
-                    g_launches++;
-                    if (int rc = scan_offsets(E, stream, toff, n)) return rc;
-                    if (int rc = split_segment(E, stream, *X, reads, off, a, n, E.trim_first.as<int64_t>(), toff, rounds, rounds.size(),
-                                               totals, Dm ? &dstage : nullptr)) return rc;
-                }
-                a = b;
-                continue;
-            }
-            // ---- trims -> trimmed reads, encoded into the middle scan's resident codes ----
-            MiddleSeg M;
-            if (int rc = middle_segment_buffers(E, n, n_mid, device ? 0 : (size_t)bytes, M)) return rc;
-            if (int rc = E.trim_first.ensure((size_t)n * 8 + 16)) return rc;
-            M.codes = E.mid_codes.as<uint8_t>();
-            M.off = E.mid_off.as<int64_t>();
-            M.cmin_len = mid_cmin_len;
-            trimmed_range_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(off, static_cast<const int32_t *>(E.trim_d[0].as<int32_t>()),
-                                                                                 static_cast<const int32_t *>(E.trim_d[1].as<int32_t>()), n,
-                                                                                 E.trim_first.as<int64_t>(), M.off);
-            g_launches++;
-            if (int rc = scan_offsets(E, stream, M.off, n)) return rc;
-            gather_encode_kernel<<<(unsigned)warp_blocks, 128, 0, stream>>>(reads, off, static_cast<const int64_t *>(E.trim_first.as<int64_t>()),
-                                                                           static_cast<const int64_t *>(M.off), n, M.codes);
-            g_launches++;
-            CK(cudaGetLastError());
-            if (int rc = device_max_len(S, stream, M.off, n, &M.max_len)) return rc;
-            // ---- Phase C: round 0 over every trimmed read, then the masking rounds, as in middle_device ----
-            CK(cudaMemsetAsync(E.mid_ctr.p, 0, 16, stream));
-            const int64_t max_cnt = std::max<int64_t>(1, g_opt.device_chunk_tasks / n_mid);
-            for (int64_t c0 = 0; c0 < n; c0 += max_cnt) {
-                const int64_t cnt = std::min(max_cnt, n - c0);
-                if (int rc = run_cross_chunk(E, S, stream, PM, M.codes, M.off + c0, cnt, 0, M.max_len, n_mid,
-                                             M.rec + (size_t)c0 * n_mid * PB_REC, nullptr, 0, A->mid_ad_off)) return rc;
-                if (int rc = launch_middle_decide(E, stream, M, n_mid, nullptr, c0, cnt, M.active[0], S.misc.as<int>())) return rc;
-            }
-            const size_t r0 = rounds.size();
-            if (int rc = middle_rounds(E, S, stream, PM, M, n_mid, A->mid_ad_off, a, rounds)) return rc;
-            if (X) {
-                if (int rc = split_segment(E, stream, *X, reads, off, a, n, E.trim_first.as<int64_t>(), M.off, rounds, r0, totals,
-                                           Dm ? &dstage : nullptr))
-                    return rc;
-            }
-            a = b;
-        }
-        if (Dm) {
-            if (int rc = demux_finalize(E, S, stream, *X, *Dm, seqs, n_seqs, totals)) return rc;
-        }
-        if (X) CK(cudaStreamSynchronize(stream));      // the device outputs are written when the call returns
         return 0;
-    };
-    const int rc = run();
-    if (rc) {                             // nothing may still be running (or writing the caller's outputs) when we return
-        const std::string first_err = g_err;
-        cudaStreamSynchronize(stream);
-        g_err = first_err;
     }
-    E.last_pending = false;               // the stream waited for an earlier call's queued work, and all of it is done
-    if (X && !rc) { *X->n_parts = totals.parts; *X->n_out_bases = totals.bases; }
+
+    // The segment's reads [a, a + n), ASCII at reads[off[s] .. off[s + 1]) -- host reads are uploaded here (their only upload),
+    // offsets rebased to the segment -- and their end windows: lengths, offsets (shared by both sides), the cut into trim_win.
+    int segment_reads(int64_t a, int64_t n, const uint8_t *&reads, const int64_t *&off) {
+        reads = seqs;
+        off = seq_off + a;
+        if (!device) {
+            const int64_t bytes = seq_off[a + n] - seq_off[a];
+            if (int rc = E.trim_reads.ensure((size_t)bytes + 16)) return rc;
+            if (int rc = E.trim_off.ensure((size_t)(n + 1) * 8)) return rc;
+            if (bytes) CK(cudaMemcpyAsync(E.trim_reads.p, seqs + seq_off[a], (size_t)bytes, cudaMemcpyHostToDevice, stream));
+            CK(cudaMemcpyAsync(E.trim_off.p, seq_off + a, (size_t)(n + 1) * 8, cudaMemcpyHostToDevice, stream));
+            rebase_kernel<<<(unsigned)((n + 1 + 255) / 256), 256, 0, stream>>>(E.trim_off.as<int64_t>(), n + 1, seq_off[a]);
+            g_launches++;
+            reads = E.trim_reads.as<uint8_t>();
+            off = E.trim_off.as<int64_t>();
+        }
+        const size_t win_bytes = (size_t)n * (size_t)wl_max;
+        if (int rc = E.trim_win_off.ensure((size_t)(n + 1) * 8)) return rc;
+        if (int rc = E.trim_win[0].ensure(win_bytes + 16)) return rc;
+        if (int rc = E.trim_win[1].ensure(win_bytes + 16)) return rc;
+        int64_t *win_off = E.trim_win_off.as<int64_t>();
+        window_len_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(off, n, (int64_t)A.end_size, win_off);
+        g_launches++;
+        if (int rc = scan_offsets(E, stream, win_off, n)) return rc;
+        const int64_t warp_blocks = std::max<int64_t>(1, std::min<int64_t>((n + 3) / 4, (int64_t)E.sm_count * 16));
+        cut_windows_kernel<<<(unsigned)warp_blocks, 128, 0, stream>>>(reads, off, static_cast<const int64_t *>(win_off), n,
+                                                                     E.trim_win[0].as<uint8_t>(), E.trim_win[1].as<uint8_t>());
+        g_launches++;
+        CK(cudaGetLastError());
+        return 0;
+    }
+
+    // Phase B of side k over the segment's reads [a, a + n): DP chunks, each followed by decide_kernel into the segment-wide
+    // trims trim_d[k].  win_total: the windows' total length, fetched (once per segment) when a side encodes them first.
+    int end_side(int k, int64_t a, int64_t n, int64_t &win_total) {
+        const pb200_trim_side_t &T = side(k);
+        if (int rc = E.trim_d[k].ensure((size_t)n * 4 + 16)) return rc;
+        if (T.n_adapters == 0) {
+            CK(cudaMemsetAsync(E.trim_d[k].p, 0, (size_t)n * 4, stream));
+            return 0;
+        }
+        const int64_t *win_off = E.trim_win_off.as<int64_t>();
+        const bool ascii = single_pass_ascii(P[k], wl_max);
+        const uint8_t *w = E.trim_win[k].as<uint8_t>();
+        if (!ascii) {                // two-pass windows: encode first, as batch_device_queue does
+            if (win_total < 0) {
+                CK(cudaMemcpyAsync(&win_total, win_off + n, 8, cudaMemcpyDeviceToHost, stream));
+                CK(cudaStreamSynchronize(stream));
+            }
+            if (int rc = S.seq_codes.ensure((size_t)win_total + 16)) return rc;
+            if (int rc = launch_encode(stream, w, S.seq_codes.as<uint8_t>(), win_total, E.sm_count)) return rc;
+            w = S.seq_codes.as<uint8_t>();
+        }
+        pb200_end_batch_t D;
+        memset(&D, 0, sizeof D);
+        D.is_start = k == 0 ? 1 : 0; D.end_size = A.end_size; D.extra_trim_size = A.extra_trim_size;
+        D.min_trim_size = A.min_trim_size; D.end_threshold = A.end_threshold;
+        D.score_cols = T.score_cols; D.n_score_cols = T.n_score_cols;
+        D.trim = T.trim; D.score_pairs = T.score_pairs; D.top2 = T.top2;
+        const int64_t max_cnt = std::max<int64_t>(1, g_opt.device_chunk_tasks / T.n_adapters);
+        int32_t *top2 = nullptr;     // demux: the segment's ranking stays on the device for barcode_call_kernel
+        if (Dm && T.n_score_cols > 0) {
+            if (int rc = E.demux_top2[k].ensure((size_t)n * 6 * 4 + 16)) return rc;
+            top2 = E.demux_top2[k].as<int32_t>();
+        }
+        for (int64_t c0 = 0; c0 < n; c0 += max_cnt) {
+            const int64_t cnt = std::min(max_cnt, n - c0);
+            if (int rc = S.out.ensure((size_t)cnt * T.n_adapters * PB_REC * 4)) return rc;
+            if (int rc = run_cross_chunk(E, S, stream, P[k], w, win_off + c0, cnt, 0, wl_max, T.n_adapters, S.out.as<int32_t>(),
+                                         nullptr, 0, T.ad_off, nullptr, ascii)) return rc;
+            if (int rc = launch_decide(E, S, stream, D, S.out.as<int32_t>(), cnt, T.n_adapters, E.dec_cmin[k].as<int32_t>(),
+                                       TP.cmin_len[k], E.dec_cols[k].as<int32_t>(), E.trim_d[k].as<int32_t>() + c0, a + c0,
+                                       top2 ? top2 + c0 * 6 : nullptr))
+                return rc;
+        }
+        return 0;
+    }
+
+    // The barcode call of every read of the segment [a, a + n), into the call-wide bins.
+    int barcode_call(int64_t a, int64_t n) {
+        const int32_t *t[2] = {nullptr, nullptr};
+        for (int k = 0; k < 2; ++k) if (side(k).n_score_cols > 0) t[k] = E.demux_top2[k].as<int32_t>();
+        barcode_call_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(
+            t[0], t[1], static_cast<const int32_t *>(E.demux_map[0].as<int32_t>()),
+            static_cast<const int32_t *>(E.demux_map[1].as<int32_t>()), static_cast<const double *>(E.demux_tab.as<double>()),
+            TP.dstage.tab_c, TP.dstage.tab_l, n, Dm->n_bins, Dm->barcode_threshold, Dm->barcode_diff, Dm->require_two_barcodes,
+            Dm->d_albacore ? Dm->d_albacore + a : nullptr, E.demux_bin.as<int32_t>() + a, S.misc.as<int>());
+        g_launches++;
+        CK(cudaGetLastError());
+        return 0;
+    }
+
+    // The trims -> every read's trimmed range: its first base in trim_first, the lengths scanned into offsets in mid_off.
+    int trimmed_ranges(const int64_t *off, int64_t n) {
+        if (int rc = E.trim_first.ensure((size_t)n * 8 + 16)) return rc;
+        if (int rc = E.mid_off.ensure((size_t)(n + 1) * 8)) return rc;
+        int64_t *toff = E.mid_off.as<int64_t>();
+        trimmed_range_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(
+            off, static_cast<const int32_t *>(E.trim_d[0].as<int32_t>()), static_cast<const int32_t *>(E.trim_d[1].as<int32_t>()),
+            n, E.trim_first.as<int64_t>(), toff);
+        g_launches++;
+        return scan_offsets(E, stream, toff, n);
+    }
+
+    // Phase C of the segment that starts at read a: the trimmed reads encoded into the middle scan's resident codes, then
+    // round 0 and the masking rounds, as in middle_device.
+    int middle_scan(const uint8_t *reads, const int64_t *off, int64_t a, MiddleSeg &M) {
+        M.codes = E.mid_codes.as<uint8_t>();
+        M.off = E.mid_off.as<int64_t>();
+        M.cmin_len = TP.mid_cmin_len;
+        const int64_t warp_blocks = std::max<int64_t>(1, std::min<int64_t>((M.n + 3) / 4, (int64_t)E.sm_count * 16));
+        gather_encode_kernel<<<(unsigned)warp_blocks, 128, 0, stream>>>(reads, off, static_cast<const int64_t *>(E.trim_first.as<int64_t>()),
+                                                                       static_cast<const int64_t *>(M.off), M.n, M.codes);
+        g_launches++;
+        CK(cudaGetLastError());
+        M.max_len = -1;
+        if (int rc = device_max_len(S, stream, M.off, M.n, &M.max_len)) return rc;
+        return middle_scan_resident(E, S, stream, PM, M, A.n_mid_adapters, A.mid_ad_off, a, rounds);
+    }
+};
+
+int trim_reads(const uint8_t *seqs, const int64_t *seq_off, int64_t n_seqs, bool device, int64_t total_seq_bytes,
+               int64_t max_seq_len, const pb200_trim_args_t *A, int ma, int mi, int go, int ge, void *user_stream,
+               const pb200_split_args_t *X = nullptr, const pb200_demux_args_t *Dm = nullptr) {
+    TrimPlan TP;
+    if (int rc = trim_plan(seqs, seq_off, n_seqs, device, total_seq_bytes, max_seq_len, A, ma, mi, go, ge, X, Dm, TP)) return rc;
+    // the host outputs the device does not write
+    if (Dm) memset(Dm->bin_parts, 0, (size_t)(Dm->n_bins + 2) * 8);
+    if (A->n_hits && n_seqs > 0) memset(A->n_hits, 0, (size_t)n_seqs * 4);
+    if (A->n_total) *A->n_total = 0;
+    for (const pb200_trim_side_t *T : {&A->start, &A->end})
+        if (T->n_adapters == 0 && n_seqs > 0) fill_no_adapters(T->trim, T->top2, n_seqs);
+    // without adapters nothing is trimmed or split; the output stage still writes every non-empty read ("No adapters found")
+    if (n_seqs == 0 || (!X && A->start.n_adapters == 0 && A->end.n_adapters == 0 && A->n_mid_adapters == 0)) return 0;
+
+    std::vector<MiddleRound> rounds;
+    SplitTotals totals;
+    const int rc = sync_call(device ? CallOn::library : CallOn::stage0, user_stream, [&](Engine &E, cudaStream_t stream) {
+        NvtxRange submit_range(Dm ? "pb200:submit_demux" : X ? "pb200:submit_trim_split" : "pb200:submit_trim");
+        TrimCall C{E, E.st[0], stream, seqs, seq_off, n_seqs, device, total_seq_bytes, *A, X, Dm, TP, rounds, totals};
+        return C.run(ma, mi, go, ge);
+    });
     if (rc) return rc;
-    if (n_mid > 0) {
-        if (int rc2 = middle_emit(rounds, n_seqs, A->n_hits, A->hits, A->hits_cap, A->n_total)) return rc2;
-    }
+    if (X) { *X->n_parts = totals.parts; *X->n_out_bases = totals.bases; }
+    if (A->n_mid_adapters > 0) { if (int rc2 = middle_emit(rounds, n_seqs, A->n_hits, A->hits, A->hits_cap, A->n_total)) return rc2; }
     if (X && totals.parts > X->parts_cap) return fail(PB200_ERR_SPACE, "parts_cap is smaller than the number of records (*n_parts)");
     return 0;
 }
@@ -2449,19 +2413,10 @@ int emit_reads(const pb200_emit_args_t *A, int64_t n_rec, void *user_stream) {
         (A->n_reads > 0 && !A->d_name_off) || (A->out_cap > 0 && !A->d_out) ||
         (n_rec > 0 && (!A->d_off || !A->d_read || !A->d_part)))
         return fail(PB200_ERR_ARG, "NULL pointer");
-
-    Engine *Ep = nullptr;
-    if (int rc = get_engine(&Ep)) return rc;
-    Engine &E = *Ep;
-    std::lock_guard<std::mutex> lk(E.mu);
-    if (int rc = E.init()) return rc;
-    Stage &S = E.st[0];
-    cudaStream_t stream = S.stream;
-    if (int rc = library_stream(E, user_stream, &stream)) return rc;
-    if (int rc = order_after_last(E, stream)) return rc;
-    NvtxRange range("pb200:emit");
-    int64_t total = 0;
-    auto run = [&]() -> int {
+    return sync_call(CallOn::library, user_stream, [&](Engine &E, cudaStream_t stream) -> int {
+        NvtxRange range("pb200:emit");
+        Stage &S = E.st[0];
+        int64_t total = 0;
         if (int rc = reset_misc(S, stream)) return rc;
         int *bad = reinterpret_cast<int *>(S.misc.as<char>() + 48);
         if (n_rec > 0) {
@@ -2493,15 +2448,7 @@ int emit_reads(const pb200_emit_args_t *A, int64_t n_rec, void *user_stream) {
             CK(cudaStreamSynchronize(stream));              // the device outputs are written when the call returns
         }
         return 0;
-    };
-    const int rc = run();
-    if (rc) {                             // nothing may still be running (or writing the caller's outputs) when we return
-        const std::string first_err = g_err;
-        cudaStreamSynchronize(stream);
-        g_err = first_err;
-    }
-    E.last_pending = false;               // the stream waited for an earlier call's queued work, and all of it is done
-    return rc;
+    });
 }
 
 }  // namespace
