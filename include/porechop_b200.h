@@ -311,6 +311,53 @@ typedef struct {
     int64_t *n_out_bytes;              /* host out, always written                                                            */
 } pb200_emit_args_t;
 int pb200EmitReadsDevice(const pb200_emit_args_t *args, int64_t n_rec, void *stream);
+/* The reads of FASTQ / FASTA bytes in device memory, parsed into caller-owned device buffers: the fields fastq.parse_fastq /
+ * fastq.parse_fasta return (the reference's loader, misc.py:123-166, and NanoporeRead.__init__, nanopore_read.py:23-36).
+ *   - Lines end at '\n'; an unterminated last line ends at n_in.  Every line is stripped of the ASCII bytes str.strip()
+ *     removes (9-13, 28-31, 32); other bytes ('\r' alone, non-ASCII) are kept.
+ *   - FASTQ (fmt 0): record r is lines 4r .. 4r+3.  The stripped header must be non-empty and start with '@'; the name is the
+ *     stripped header minus that byte, the bases are line 4r+1, the qualities line 4r+3 (line 4r+2 is not looked at).
+ *   - FASTA (fmt 1): blank lines are dropped; the first kept line must start with '>'; every '>' line starts a record whose
+ *     name is the line minus '>' (never empty), and the record's bases are its body lines concatenated.
+ *   - Bases are upper-cased (a-z only); d_rna[r] = 1 when the read has more 'U' than 'T' bytes, and such a read stores every
+ *     'U' as 'T'.
+ *   - d_qual (optional) gets one quality per base at the bases' offsets: FASTQ qualities padded with '+' to the bases' length,
+ *     FASTA '+' for every base.
+ * d_name_off / d_seq_off get n_reads + 1 offsets (0 first).  n_reads, n_name_bytes and n_seq_bytes are always written.  When
+ * a count exceeds its capacity the call returns PB200_ERR_SPACE with the exact counts and writes no device output.
+ * Malformed input returns PB200_ERR_ARG with *error set (PB200_PARSE_*) and *error_index = the first bad FASTQ record or FASTA
+ * line (0-based); no device output is written.  A FASTQ quality line longer than its bases cannot be held at the bases'
+ * offsets: with d_qual set that is PB200_PARSE_LONG_QUAL (callers parse such a chunk on the host).  Empty input gives 0 reads
+ * without a kernel launch.  The call returns once the device outputs are written; stream and ordering rules as
+ * pb200EmitReadsDevice.
+ * Preconditions, checked before the device is touched (PB200_ERR_ARG, *error 0): args not NULL, fmt 0 or 1, no negative
+ * size, every host output, d_name_off and d_seq_off, and the device pointers whose capacity is nonzero. */
+enum {
+    PB200_PARSE_OK = 0,
+    PB200_PARSE_LINES = 1,       /* FASTQ: the number of lines is not a multiple of 4 (index: the incomplete record)       */
+    PB200_PARSE_HEADER = 2,      /* FASTQ: a stripped header is empty or does not start with '@'                          */
+    PB200_PARSE_FASTA_START = 3, /* FASTA: a body line comes before the first '>' line                                     */
+    PB200_PARSE_FASTA_NAME = 4,  /* FASTA: a '>' line with an empty name                                                   */
+    PB200_PARSE_LONG_QUAL = 5    /* FASTQ with d_qual: a quality line longer than its bases                               */
+};
+typedef struct {
+    const uint8_t *d_in;               /* device, n_in bytes of whole records                                                 */
+    int64_t n_in;
+    int32_t fmt;                       /* 0 = FASTQ, 1 = FASTA                                                                */
+    uint8_t *d_names;                  /* device out, names_cap bytes: read r's name at d_name_off[r] .. d_name_off[r + 1]    */
+    int64_t names_cap;
+    int64_t *d_name_off;               /* device out, reads_cap + 1                                                           */
+    uint8_t *d_seq;                    /* device out, seq_cap bytes: read r's bases at d_seq_off[r] .. d_seq_off[r + 1]       */
+    int64_t seq_cap;
+    int64_t *d_seq_off;                /* device out, reads_cap + 1                                                           */
+    uint8_t *d_qual;                   /* device out, seq_cap bytes at the bases' offsets, or NULL: no qualities              */
+    uint8_t *d_rna;                    /* device out, reads_cap: 1 = RNA read                                                 */
+    int64_t reads_cap;
+    int64_t *n_reads, *n_name_bytes, *n_seq_bytes;   /* host out, always written                                             */
+    int32_t *error;                    /* host out: PB200_PARSE_* (0 unless malformed input)                                  */
+    int64_t *error_index;              /* host out: first bad record (FASTQ) or line (FASTA), -1 when none                    */
+} pb200_parse_args_t;
+int pb200ParseReadsDevice(const pb200_parse_args_t *args, void *stream);
 /* cmin[l], l = 0 .. len-1: the smallest c with float("%f" % (100.0*c/l)) >= middle_threshold, or l+1 if none does
  * (cmin[0] = INT32_MAX).  The ">=" sibling of pb200TrimThresholdTable.  Pure host code; middle_threshold must be > 0. */
 int pb200MiddleThresholdTable(double middle_threshold, int32_t len, int32_t *cmin);

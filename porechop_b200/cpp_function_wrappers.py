@@ -135,6 +135,18 @@ class EmitArgsDesc(Structure):
 
 C_LIB.pb200EmitReadsDevice.argtypes = [POINTER(EmitArgsDesc), c_int64, c_void_p]
 C_LIB.pb200EmitReadsDevice.restype = c_int
+
+
+class ParseArgsDesc(Structure):
+    """pb200_parse_args_t (include/porechop_b200.h)"""
+    _fields_ = [('d_in', c_void_p), ('n_in', c_int64), ('fmt', c_int32), ('d_names', c_void_p), ('names_cap', c_int64),
+                ('d_name_off', c_void_p), ('d_seq', c_void_p), ('seq_cap', c_int64), ('d_seq_off', c_void_p), ('d_qual', c_void_p),
+                ('d_rna', c_void_p), ('reads_cap', c_int64), ('n_reads', c_void_p), ('n_name_bytes', c_void_p),
+                ('n_seq_bytes', c_void_p), ('error', c_void_p), ('error_index', c_void_p)]
+
+
+C_LIB.pb200ParseReadsDevice.argtypes = [POINTER(ParseArgsDesc), c_void_p]
+C_LIB.pb200ParseReadsDevice.restype = c_int
 C_LIB.pb200MiddleThresholdTable.argtypes = [c_double, c_int32, c_void_p]
 C_LIB.pb200MiddleThresholdTable.restype = c_int
 C_LIB.pb200FormatRecord.argtypes = [c_void_p, c_char_p, c_int]
@@ -160,7 +172,7 @@ EXPORTED_SYMBOLS = ['adapterAlignment', 'freeCString', 'adapterAlignmentBatch', 
                     'adapterAlignmentBatchDevice', 'adapterEndDecisions', 'pb200TrimThresholdTable', 'adapterSetSearch',
                     'adapterMiddleScan',
                     'adapterMiddleScanDevice', 'pb200MiddleThresholdTable', 'adapterTrimReads', 'adapterTrimReadsDevice',
-                    'adapterTrimSplitReadsDevice', 'adapterDemuxReadsDevice', 'pb200EmitReadsDevice', 'pb200FormatRecord', 'pb200DeviceCount', 'pb200SetDevice', 'pb200Synchronize', 'pb200LastError',
+                    'adapterTrimSplitReadsDevice', 'adapterDemuxReadsDevice', 'pb200EmitReadsDevice', 'pb200ParseReadsDevice', 'pb200FormatRecord', 'pb200DeviceCount', 'pb200SetDevice', 'pb200Synchronize', 'pb200LastError',
                     'pb200KernelLaunches', 'pb200TimingEnable', 'pb200TimingRead', 'pb200TimingReadKinds', 'pb200SetOption',
                     'pb200GetOption', 'pb200HostBuffer', 'pb200PackNibbles']
 
@@ -593,6 +605,34 @@ def pb200_emit_reads_device(n_rec, *, d_seq_ptr, d_qual_ptr, seq_bytes, d_off_pt
         e.n_out_bytes = n_out.value
         raise
     return n_out.value
+
+
+# reason codes of pb200ParseReadsDevice (PB200_PARSE_*)
+PARSE_LINES, PARSE_HEADER, PARSE_FASTA_START, PARSE_FASTA_NAME, PARSE_LONG_QUAL = 1, 2, 3, 4, 5
+
+
+def pb200_parse_reads_device(d_in_ptr, n_in, fmt='fastq', *, d_names_ptr=0, names_cap=0, d_name_off_ptr=0, d_seq_ptr=0, seq_cap=0,
+                             d_seq_off_ptr=0, d_qual_ptr=0, d_rna_ptr=0, reads_cap=0, stream_ptr=0):
+    """The reads of n_in FASTQ / FASTA bytes in device memory (pb200ParseReadsDevice) into caller-owned device buffers: names
+    (names_cap bytes) at name_off (int64[reads_cap + 1]), bases (seq_cap bytes) and, with d_qual_ptr, qualities at seq_off
+    (int64[reads_cap + 1]), and one RNA flag (uint8) per read.  fmt: 'fastq' or 'fasta'.
+    Returns (n_reads, name bytes, bases).  When they do not fit it raises EngineError with code ERR_SPACE and the exact counts as
+    .n_reads / .n_name_bytes / .n_seq_bytes; malformed input raises EngineError with code ERR_ARG, .reason (PARSE_*) and .index
+    (the first bad record or line)."""
+    if fmt not in ('fastq', 'fasta'):
+        raise ValueError("fmt must be 'fastq' or 'fasta'")
+    outs = [c_int64(0) for _ in range(3)]
+    err, err_index = c_int32(0), c_int64(-1)
+    args = ParseArgsDesc(d_in_ptr or None, int(n_in), 0 if fmt == 'fastq' else 1, d_names_ptr or None, int(names_cap),
+                         d_name_off_ptr or None, d_seq_ptr or None, int(seq_cap), d_seq_off_ptr or None, d_qual_ptr or None,
+                         d_rna_ptr or None, int(reads_cap), *(addressof(x) for x in outs), addressof(err), addressof(err_index))
+    try:
+        _check(C_LIB.pb200ParseReadsDevice(byref(args), c_void_p(stream_ptr)))
+    except EngineError as e:
+        e.n_reads, e.n_name_bytes, e.n_seq_bytes = (x.value for x in outs)
+        e.reason, e.index = err.value, err_index.value
+        raise
+    return tuple(x.value for x in outs)
 
 
 def middle_threshold_table(middle_threshold, length):

@@ -206,6 +206,9 @@ struct Engine {
     // once never share an accumulator; a batch owns the columns [search_col, search_col + n_adapters) of every slice
     DevBuf search_acc;
     int64_t search_cols = 0;
+    // parse (pb200ParseReadsDevice): line counts per tile (scanned), line ends, the per-record (FASTQ) or per-line (FASTA) index
+    // arrays, and one status byte per record or line
+    DevBuf parse_tiles, parse_lines, parse_index, parse_status;
     std::shared_ptr<void> packer;        // Packer (below): the thread that plans and packs chunks ahead of the submit loop
     // Ordering between calls: every entry point uses the stage buffers above (st[0]'s trace scratch, tasks, codes, status word),
     // whatever stream it runs on.  A call that returns with work still queued (adapterAlignmentBatchDevice) records `last` on
@@ -770,7 +773,7 @@ int check_status(Stage &S, cudaStream_t stream) {
 }
 
 // S.misc: status word at offset 0, score-pass counter at 16, max-length scratch at 32, pb200EmitReadsDevice's record-check flag
-// at 48.  The status word is sticky until
+// at 48, pb200ParseReadsDevice's check flags at 56.  The status word is sticky until
 // pb200Synchronize, which reports and clears it: a deferred error of an earlier device-resident call must not be lost, so a
 // call clears the word only when it allocates it, and everything behind it always.
 int reset_misc(Stage &S, cudaStream_t stream) {
@@ -2451,6 +2454,145 @@ int emit_reads(const pb200_emit_args_t *A, int64_t n_rec, void *user_stream) {
     });
 }
 
+// ---- parsing (pb200ParseReadsDevice) -----------------------------------------------------------------------------------
+// The lines are counted per tile and the count comes home (it sizes the line index); the line ends, the record or line index
+// and its scans follow, and the counts, totals and check flags come home in one synchronise.  When the input is well formed
+// and everything fits, the offsets are copied out and one warp per record (FASTQ) or line (FASTA) writes the bytes; one warp
+// per read then normalises the bases.
+int parse_reads(const pb200_parse_args_t *A, void *user_stream) {
+    if (!A) return fail(PB200_ERR_ARG, "NULL pointer");
+    for (int64_t *p : {A->n_reads, A->n_name_bytes, A->n_seq_bytes}) if (p) *p = 0;
+    if (A->error) *A->error = PB200_PARSE_OK;
+    if (A->error_index) *A->error_index = -1;
+    if (!A->n_reads || !A->n_name_bytes || !A->n_seq_bytes || !A->error || !A->error_index) return fail(PB200_ERR_ARG, "NULL pointer");
+    if (A->fmt != 0 && A->fmt != 1) return fail(PB200_ERR_ARG, "fmt must be 0 (FASTQ) or 1 (FASTA)");
+    if (A->n_in < 0 || A->names_cap < 0 || A->seq_cap < 0 || A->reads_cap < 0) return fail(PB200_ERR_ARG, "negative count");
+    if ((A->n_in > 0 && !A->d_in) || !A->d_name_off || !A->d_seq_off || (A->names_cap > 0 && !A->d_names) ||
+        (A->seq_cap > 0 && !A->d_seq) || (A->reads_cap > 0 && !A->d_rna))
+        return fail(PB200_ERR_ARG, "NULL pointer");
+    const int64_t n = A->n_in;
+    const bool fastq = A->fmt == 0;
+    return sync_call(CallOn::library, user_stream, [&](Engine &E, cudaStream_t stream) -> int {
+        NvtxRange range("pb200:parse");
+        if (n == 0) {                                      // no reads: the offsets' first entries only
+            CK(cudaMemsetAsync(A->d_name_off, 0, 8, stream));
+            CK(cudaMemsetAsync(A->d_seq_off, 0, 8, stream));
+            CK(cudaStreamSynchronize(stream));
+            return 0;
+        }
+        Stage &S = E.st[0];
+        if (int rc = reset_misc(S, stream)) return rc;
+        int *flags = reinterpret_cast<int *>(S.misc.as<char>() + 56);
+        // ---- the line index ----
+        const int64_t tiles = (n + PB_PARSE_TILE - 1) / PB_PARSE_TILE;
+        if (int rc = E.parse_tiles.ensure((size_t)(tiles + 1) * 8)) return rc;
+        int64_t *first_line = E.parse_tiles.as<int64_t>();
+        parse_count_lines_kernel<<<(unsigned)tiles, PB_PARSE_THREADS, 0, stream>>>(A->d_in, n, first_line);
+        g_launches++;
+        CK(cudaGetLastError());
+        if (int rc = scan_offsets(E, stream, first_line, tiles)) return rc;
+        int64_t n_nl = 0;
+        uint8_t last = 0;
+        CK(cudaMemcpyAsync(&n_nl, first_line + tiles, 8, cudaMemcpyDeviceToHost, stream));
+        CK(cudaMemcpyAsync(&last, A->d_in + n - 1, 1, cudaMemcpyDeviceToHost, stream));
+        CK(cudaStreamSynchronize(stream));
+        const int64_t n_lines = n_nl + (last != '\n');
+        if (fastq && n_lines % 4 != 0) {
+            *A->error = PB200_PARSE_LINES;
+            *A->error_index = n_lines / 4;
+            return fail(PB200_ERR_ARG, "FASTQ chunk is not a whole number of 4-line records");
+        }
+        if (int rc = E.parse_lines.ensure((size_t)n_lines * 8)) return rc;
+        int64_t *line_end = E.parse_lines.as<int64_t>();
+        parse_line_ends_kernel<<<(unsigned)tiles, PB_PARSE_THREADS, 0, stream>>>(A->d_in, n, static_cast<const int64_t *>(first_line),
+                                                                                 line_end);
+        g_launches++;
+        CK(cudaGetLastError());
+        // ---- records (FASTQ) or lines (FASTA): spans, checks, lengths scanned into offsets ----
+        const int64_t m = fastq ? n_lines / 4 : n_lines;   // index entries: records or lines
+        if (int rc = E.parse_index.ensure((size_t)(m + 1) * 8 * 7)) return rc;
+        if (int rc = E.parse_status.ensure((size_t)m)) return rc;
+        int64_t *ix = E.parse_index.as<int64_t>();
+        int64_t *col[7];
+        for (int c = 0; c < 7; ++c) col[c] = ix + (size_t)c * (m + 1);
+        uint8_t *status = E.parse_status.as<uint8_t>();
+        const unsigned grid = (unsigned)std::max<int64_t>(1, (m + 255) / 256);
+        // FASTQ: name_a, name_off, seq_a, seq_off, qual_a, qual_len.  FASTA: span_a, span_len, hdr, nm, body, name_off, seq_off.
+        int64_t *name_off = fastq ? col[1] : col[5], *seq_off = fastq ? col[3] : col[6];
+        int64_t tot[3] = {0, 0, 0};                        // reads, name bytes, bases
+        if (fastq) {
+            parse_fastq_index_kernel<<<grid, 256, 0, stream>>>(A->d_in, static_cast<const int64_t *>(line_end), m, A->d_qual != nullptr,
+                                                               col[0], col[1], col[2], col[3], col[4], col[5], status, flags);
+            g_launches++;
+            CK(cudaGetLastError());
+            if (int rc = scan_offsets(E, stream, name_off, m)) return rc;
+            if (int rc = scan_offsets(E, stream, seq_off, m)) return rc;
+            tot[0] = m;
+        } else {
+            parse_fasta_lines_kernel<<<grid, 256, 0, stream>>>(A->d_in, static_cast<const int64_t *>(line_end), m, col[0], col[1],
+                                                               col[2], col[3], col[4]);
+            g_launches++;
+            CK(cudaGetLastError());
+            for (int c = 2; c < 5; ++c)
+                if (int rc = scan_offsets(E, stream, col[c], m)) return rc;
+            parse_fasta_records_kernel<<<grid, 256, 0, stream>>>(col[1], col[2], col[3], col[4], A->d_in, col[0], m, name_off, seq_off,
+                                                                 status, flags);
+            g_launches++;
+            CK(cudaGetLastError());
+            CK(cudaMemcpyAsync(&tot[0], col[2] + m, 8, cudaMemcpyDeviceToHost, stream));
+        }
+        int st[2] = {0, 0};
+        CK(cudaMemcpyAsync(&tot[1], (fastq ? name_off : col[3]) + m, 8, cudaMemcpyDeviceToHost, stream));
+        CK(cudaMemcpyAsync(&tot[2], (fastq ? seq_off : col[4]) + m, 8, cudaMemcpyDeviceToHost, stream));
+        CK(cudaMemcpyAsync(&st[0], S.misc.p, 4, cudaMemcpyDeviceToHost, stream));
+        CK(cudaMemcpyAsync(&st[1], flags, 4, cudaMemcpyDeviceToHost, stream));
+        CK(cudaStreamSynchronize(stream));
+        *A->n_reads = tot[0];
+        *A->n_name_bytes = tot[1];
+        *A->n_seq_bytes = tot[2];
+        if (int rc = status_error(st[0])) return rc;       // a deferred error of an earlier device-resident call
+        if (st[1]) {                                       // malformed input: the first record / line of the first failing check
+            const int bad = (st[1] & 2) ? 1 : 2;
+            std::vector<uint8_t> h((size_t)m);
+            CK(cudaMemcpyAsync(h.data(), status, (size_t)m, cudaMemcpyDeviceToHost, stream));
+            CK(cudaStreamSynchronize(stream));
+            *A->error_index = std::find(h.begin(), h.end(), (uint8_t)bad) - h.begin();
+            if (fastq) {
+                *A->error = bad == 1 ? PB200_PARSE_HEADER : PB200_PARSE_LONG_QUAL;
+                return fail(PB200_ERR_ARG, bad == 1 ? "FASTQ record does not start with @"
+                                                    : "a quality line is longer than its bases (parse this chunk on the host)");
+            }
+            *A->error = bad == 1 ? PB200_PARSE_FASTA_START : PB200_PARSE_FASTA_NAME;
+            return fail(PB200_ERR_ARG, bad == 1 ? "FASTA does not start with a > line" : "FASTA record with an empty name");
+        }
+        if (tot[0] > A->reads_cap || tot[1] > A->names_cap || tot[2] > A->seq_cap)
+            return fail(PB200_ERR_SPACE, "reads_cap, names_cap or seq_cap is smaller than the parse (*n_reads, *n_name_bytes, *n_seq_bytes)");
+        // ---- the outputs ----
+        const int64_t r = tot[0];
+        CK(cudaMemcpyAsync(A->d_name_off, name_off, (size_t)(r + 1) * 8, cudaMemcpyDeviceToDevice, stream));
+        CK(cudaMemcpyAsync(A->d_seq_off, seq_off, (size_t)(r + 1) * 8, cudaMemcpyDeviceToDevice, stream));
+        const int64_t blocks = std::max<int64_t>(1, std::min<int64_t>((m + 7) / 8, (int64_t)E.sm_count * 8));
+        if (fastq) {
+            parse_fastq_write_kernel<<<(unsigned)blocks, 256, 0, stream>>>(A->d_in, col[0], name_off, col[2], seq_off, col[4], col[5], m,
+                                                                           A->d_names, A->d_seq, A->d_qual);
+        } else {
+            parse_fasta_write_kernel<<<(unsigned)blocks, 256, 0, stream>>>(A->d_in, col[0], col[1], col[3], col[4], m, A->d_names,
+                                                                           A->d_seq);
+            if (A->d_qual && tot[2] > 0) CK(cudaMemsetAsync(A->d_qual, '+', (size_t)tot[2], stream));
+        }
+        g_launches++;
+        CK(cudaGetLastError());
+        if (r > 0) {
+            const int64_t nb = std::max<int64_t>(1, std::min<int64_t>((r + 7) / 8, (int64_t)E.sm_count * 8));
+            parse_normalise_kernel<<<(unsigned)nb, 256, 0, stream>>>(static_cast<const int64_t *>(A->d_seq_off), r, A->d_seq, A->d_rna);
+            g_launches++;
+            CK(cudaGetLastError());
+        }
+        CK(cudaStreamSynchronize(stream));                 // the device outputs are written when the call returns
+        return 0;
+    });
+}
+
 }  // namespace
 
 // =====================================================================================================
@@ -2537,6 +2679,11 @@ int adapterDemuxReadsDevice(const uint8_t *d_seqs, const int64_t *d_seq_off, int
 int pb200EmitReadsDevice(const pb200_emit_args_t *args, int64_t n_rec, void *stream) {
     g_err.clear();
     return emit_reads(args, n_rec, stream);
+}
+
+int pb200ParseReadsDevice(const pb200_parse_args_t *args, void *stream) {
+    g_err.clear();
+    return parse_reads(args, stream);
 }
 
 int pb200MiddleThresholdTable(double middle_threshold, int32_t len, int32_t *cmin) {

@@ -1385,6 +1385,203 @@ __global__ void __launch_bounds__(256) emit_write_kernel(const uint8_t *seq, con
 }
 
 // ---------------------------------------------------------------------------------------------------
+// pb200ParseReadsDevice: FASTQ / FASTA bytes -> names, bases, qualities and RNA flags (fastq.parse_fastq / parse_fasta).
+// The line index is one tile of PB_PARSE_TILE input bytes per block, 32 contiguous bytes per thread: parse_count_lines_kernel
+// counts the '\n' bytes of every tile, scan_offsets turns the counts into each tile's first line, and parse_line_ends_kernel
+// scatters every line's end (an unterminated last line ends at n).  Records (FASTQ) or lines (FASTA) are then stripped,
+// checked and measured one per thread; scan_offsets places them; one warp per record or line copies the bytes.
+constexpr int PB_PARSE_THREADS = 256;
+constexpr int64_t PB_PARSE_TILE = (int64_t)PB_PARSE_THREADS * 32;
+
+// what str.strip() removes from an ASCII line (is_ws of hostio.c)
+__device__ __forceinline__ bool parse_ws(uint8_t c) { return c == ' ' || (c >= 9 && c <= 13) || (c >= 28 && c <= 31); }
+__device__ __forceinline__ void parse_strip(const uint8_t *buf, int64_t &a, int64_t &b) {
+    while (b > a && parse_ws(buf[b - 1])) --b;
+    while (a < b && parse_ws(buf[a])) ++a;
+}
+// the 32 input bytes of this thread (zero past n): two 16-byte loads when they are whole and aligned
+__device__ __forceinline__ void parse_load32(const uint8_t *buf, int64_t n, int64_t p, unsigned w[8]) {
+    if (p + 32 <= n && (((uintptr_t)(buf + p)) & 15) == 0) {
+        const uint4 *v = reinterpret_cast<const uint4 *>(buf + p);
+        const uint4 x = v[0], y = v[1];
+        w[0] = x.x; w[1] = x.y; w[2] = x.z; w[3] = x.w; w[4] = y.x; w[5] = y.y; w[6] = y.z; w[7] = y.w;
+        return;
+    }
+    for (int k = 0; k < 8; ++k) {
+        unsigned u = 0;
+        for (int j = 0; j < 4; ++j)
+            if (p + 4 * k + j < n) u |= (unsigned)buf[p + 4 * k + j] << (8 * j);
+        w[k] = u;
+    }
+}
+__device__ __forceinline__ int parse_count_nl(const unsigned w[8]) {
+    int c = 0;
+#pragma unroll
+    for (int k = 0; k < 8; ++k)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) c += ((w[k] >> (8 * j)) & 0xff) == '\n';
+    return c;
+}
+// cnt[t + 1] = the '\n' bytes of tile t (cnt[0] = 0), for scan_offsets
+__global__ void __launch_bounds__(PB_PARSE_THREADS) parse_count_lines_kernel(const uint8_t *buf, int64_t n, int64_t *cnt) {
+    const int64_t p = (int64_t)blockIdx.x * PB_PARSE_TILE + (int64_t)threadIdx.x * 32;
+    unsigned w[8];
+    parse_load32(buf, n, p, w);
+    long long total = 0;
+    block_exclusive_scan(parse_count_nl(w), &total);
+    if (threadIdx.x == 0) {
+        cnt[blockIdx.x + 1] = total;
+        if (blockIdx.x == 0) cnt[0] = 0;
+    }
+}
+// line_end[k] = the position of the k-th '\n' (first_line[t]: lines before tile t, scanned); the unterminated last line, if any,
+// ends at n: its index is first_line[tiles], the number of '\n' bytes
+__global__ void __launch_bounds__(PB_PARSE_THREADS) parse_line_ends_kernel(const uint8_t *buf, int64_t n, const int64_t *first_line,
+                                                                           int64_t *line_end) {
+    const int64_t p = (int64_t)blockIdx.x * PB_PARSE_TILE + (int64_t)threadIdx.x * 32;
+    unsigned w[8];
+    parse_load32(buf, n, p, w);
+    long long total = 0;
+    int64_t k = first_line[blockIdx.x] + block_exclusive_scan(parse_count_nl(w), &total);
+#pragma unroll
+    for (int i = 0; i < 8; ++i)
+#pragma unroll
+        for (int j = 0; j < 4; ++j)
+            if (((w[i] >> (8 * j)) & 0xff) == '\n') line_end[k++] = p + 4 * i + j;
+    if (p <= n - 1 && n - 1 < p + 32 && buf[n - 1] != '\n') line_end[first_line[gridDim.x]] = n;
+}
+
+// FASTQ, one thread per record: the stripped header (name = header minus '@'), bases and qualities; name_len / seq_len at [r + 1]
+// ([0] = 0) for scan_offsets.  status[r]: 1 = the header is empty or lacks '@', 2 = qualities longer than the bases (checked when
+// want_qual), else 0; *flags gets 1 << status.
+__global__ void parse_fastq_index_kernel(const uint8_t *buf, const int64_t *line_end, int64_t n_rec, int want_qual,
+                                         int64_t *name_a, int64_t *name_len, int64_t *seq_a, int64_t *seq_len, int64_t *qual_a,
+                                         int64_t *qual_len, uint8_t *status, int *flags) {
+    const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (r == 0) { name_len[0] = 0; seq_len[0] = 0; }
+    if (r >= n_rec) return;
+    const int64_t k = 4 * r;
+    int64_t a0 = k ? line_end[k - 1] + 1 : 0, b0 = line_end[k];
+    int64_t a1 = line_end[k] + 1, b1 = line_end[k + 1];
+    int64_t a3 = line_end[k + 2] + 1, b3 = line_end[k + 3];
+    parse_strip(buf, a0, b0);
+    parse_strip(buf, a1, b1);
+    parse_strip(buf, a3, b3);
+    const bool head_ok = b0 > a0 && buf[a0] == '@';
+    const uint8_t st = !head_ok ? 1 : (want_qual && b3 - a3 > b1 - a1) ? 2 : 0;
+    status[r] = st;
+    if (st) atomicOr(flags, 1 << st);
+    name_a[r] = a0 + 1;
+    name_len[r + 1] = head_ok ? b0 - a0 - 1 : 0;
+    seq_a[r] = a1;
+    seq_len[r + 1] = b1 - a1;
+    qual_a[r] = a3;
+    qual_len[r] = b3 - a3;
+}
+// FASTA, one thread per line: the stripped span, and at [l + 1] ([0] = 0) for scan_offsets: 1 for a '>' line (hdr), the name
+// length of a '>' line (nm) and the length of a kept body line (body)
+__global__ void parse_fasta_lines_kernel(const uint8_t *buf, const int64_t *line_end, int64_t n_lines, int64_t *span_a,
+                                         int64_t *span_len, int64_t *hdr, int64_t *nm, int64_t *body) {
+    const int64_t l = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (l == 0) { hdr[0] = 0; nm[0] = 0; body[0] = 0; }
+    if (l >= n_lines) return;
+    int64_t a = l ? line_end[l - 1] + 1 : 0, b = line_end[l];
+    parse_strip(buf, a, b);
+    const int64_t len = b - a;
+    const bool head = len > 0 && buf[a] == '>';
+    span_a[l] = a;
+    span_len[l] = len;
+    hdr[l + 1] = head;
+    nm[l + 1] = head ? len - 1 : 0;
+    body[l + 1] = head ? 0 : len;
+}
+// FASTA, one thread per line, after the scans (hdr[l] = records before line l): record hdr[l] of a '>' line starts at names
+// nm[l] and bases body[l]; the end offsets go after the last record.  status[l]: 1 = a body line before the first '>' line,
+// 2 = a '>' line with an empty name, else 0; *flags gets 1 << status.
+__global__ void parse_fasta_records_kernel(const int64_t *span_len, const int64_t *hdr, const int64_t *nm, const int64_t *body,
+                                           const uint8_t *buf, const int64_t *span_a, int64_t n_lines, int64_t *name_off,
+                                           int64_t *seq_off, uint8_t *status, int *flags) {
+    const int64_t l = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (l == 0) {
+        name_off[hdr[n_lines]] = nm[n_lines];
+        seq_off[hdr[n_lines]] = body[n_lines];
+    }
+    if (l >= n_lines) return;
+    const int64_t len = span_len[l];
+    const bool head = len > 0 && buf[span_a[l]] == '>';
+    uint8_t st = 0;
+    if (head) {
+        name_off[hdr[l]] = nm[l];
+        seq_off[hdr[l]] = body[l];
+        if (len < 2) st = 2;
+    } else if (len > 0 && hdr[l] == 0) {
+        st = 1;
+    }
+    status[l] = st;
+    if (st) atomicOr(flags, 1 << st);
+}
+
+struct CopyUpper {  // a-z -> A-Z, nothing else changes (NanoporeRead.__init__: seq.upper() of ASCII bases)
+    __device__ __forceinline__ unsigned operator()(unsigned w) const {
+        const unsigned h = w & 0x7f7f7f7fu;
+        const unsigned ge_a = h + 0x1f1f1f1fu, gt_z = h + 0x05050505u;     // high bit: byte >= 'a', byte > 'z'
+        const unsigned m = ge_a & ~gt_z & ~w & 0x80808080u;                  // ASCII lower-case letters
+        return w - (m >> 2);                                                  // -0x20 in those bytes (no borrow)
+    }
+};
+// FASTQ, one warp per record: the name, the upper-cased bases and (qual not NULL) the qualities, padded with '+' to the bases'
+// length (every check passed, so no quality line is longer than its bases)
+__global__ void __launch_bounds__(256) parse_fastq_write_kernel(const uint8_t *buf, const int64_t *name_a, const int64_t *name_off,
+                                                                const int64_t *seq_a, const int64_t *seq_off, const int64_t *qual_a,
+                                                                const int64_t *qual_len, int64_t n_rec, uint8_t *names,
+                                                                uint8_t *seq, uint8_t *qual) {
+    const int lane = threadIdx.x & 31;
+    const int64_t warps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    for (int64_t r = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; r < n_rec; r += warps) {
+        const int64_t s0 = seq_off[r], sl = seq_off[r + 1] - s0;
+        warp_copy(buf + name_a[r], names + name_off[r], name_off[r + 1] - name_off[r], lane);
+        warp_copy(buf + seq_a[r], seq + s0, sl, lane, CopyUpper());
+        if (qual) {
+            const int64_t ql = qual_len[r] < sl ? qual_len[r] : sl;
+            warp_copy(buf + qual_a[r], qual + s0, ql, lane);
+            for (int64_t j = ql + lane; j < sl; j += 32) qual[s0 + j] = '+';
+        }
+    }
+}
+// FASTA, one warp per kept line: a '>' line's name to names + nm[l], a body line's upper-cased bases to seq + body[l]
+__global__ void __launch_bounds__(256) parse_fasta_write_kernel(const uint8_t *buf, const int64_t *span_a, const int64_t *span_len,
+                                                                const int64_t *nm, const int64_t *body, int64_t n_lines,
+                                                                uint8_t *names, uint8_t *seq) {
+    const int lane = threadIdx.x & 31;
+    const int64_t warps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    for (int64_t l = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; l < n_lines; l += warps) {
+        const int64_t len = span_len[l];
+        if (len == 0) continue;
+        const uint8_t *src = buf + span_a[l];
+        if (*src == '>') warp_copy(src + 1, names + nm[l], len - 1, lane);
+        else warp_copy(src, seq + body[l], len, lane, CopyUpper());
+    }
+}
+// one warp per read of the written (upper-cased) bases: rna[r] = count('U') > count('T'), and an RNA read's 'U' become 'T'
+__global__ void __launch_bounds__(256) parse_normalise_kernel(const int64_t *seq_off, int64_t n_rec, uint8_t *seq, uint8_t *rna) {
+    const int lane = threadIdx.x & 31;
+    const int64_t warps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    for (int64_t r = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; r < n_rec; r += warps) {
+        const int64_t s0 = seq_off[r], sl = seq_off[r + 1] - s0;
+        long long d = 0;                                           // count('U') - count('T') of this lane's bytes
+        for (int64_t j = lane; j < sl; j += 32) {
+            const uint8_t c = seq[s0 + j];
+            d += (c == 'U') - (c == 'T');
+        }
+        for (int o = 16; o > 0; o >>= 1) d += __shfl_xor_sync(0xffffffffu, d, o);
+        if (lane == 0) rna[r] = d > 0;
+        if (d > 0)
+            for (int64_t j = lane; j < sl; j += 32)
+                if (seq[s0 + j] == 'U') seq[s0 + j] = 'T';
+    }
+}
+
+// ---------------------------------------------------------------------------------------------------
 // Demux stage of adapterDemuxReadsDevice.  Per segment, barcode_call_kernel turns the two sides' top-2 rankings (decide_kernel)
 // into each read's bin.  Once per call, after the last segment, the records the output stage placed in read order (engine
 // scratch: source offset, offsets, read, part) are partitioned stably by key = their read's bin ('none' = n_bins, or

@@ -74,6 +74,23 @@ class TorchDevice:
     def host(self, t):
         return t.cpu().numpy()
 
+    def upload_bytes(self, data):
+        """host bytes -> a uint8 CUDA tensor, through a pinned staging tensor (the upload is then plain DMA)"""
+        torch = self.torch
+        src = np.frombuffer(data, dtype=np.uint8) if not isinstance(data, np.ndarray) else np.ascontiguousarray(data).view(np.uint8)
+        out = torch.empty(len(src), dtype=torch.uint8, device='cuda')
+        if len(src):
+            staged = torch.empty(len(src), dtype=torch.uint8, pin_memory=True)
+            staged.numpy()[:] = src
+            out.copy_(staged, non_blocking=True)
+        return out
+
+    def download(self, t):
+        """a device tensor -> host numpy array, through a pinned tensor (one copy)"""
+        staged = self.torch.empty(t.numel(), dtype=t.dtype, pin_memory=True)
+        staged.copy_(t)
+        return staged.numpy()
+
     def check(self, seq, seq_off, qual):
         torch = self.torch
         for name, t, dt in (('seq', seq, torch.uint8), ('seq_off', seq_off, torch.int64), ('qual', qual, torch.uint8)):
@@ -83,6 +100,10 @@ class TorchDevice:
                 raise ValueError('%s must be a contiguous 1-D %s CUDA tensor' % (name, dt))
         if qual is not None and qual.numel() != seq.numel():
             raise ValueError('qual must hold one quality per base, at the offsets of the reads')
+
+    def check_bytes(self, data):
+        if not (data.is_cuda and data.dtype == self.torch.uint8 and data.dim() == 1 and data.is_contiguous()):
+            raise ValueError('data must be a contiguous 1-D torch.uint8 CUDA tensor')
 
     def check_names(self, names, name_off, rna):
         torch = self.torch
@@ -280,3 +301,173 @@ def emit_reads(out, names, name_off, rna=None, fmt='fastq'):
         o = D.host(off)
         bins = {name: (int(o[r0]), int(o[r1])) for name, (r0, r1) in out.bins.items()}
     return EmittedReads(D.head(data, n_out), off, bins)
+
+
+# ---- bytes in: FASTQ / FASTA parsed on the device, and whole chunks from input bytes to output bytes ------------------------
+ParsedReads = collections.namedtuple('ParsedReads', 'names name_off seq seq_off qual rna kind')
+
+_PARSE_MESSAGES = {W.PARSE_LINES: 'FASTQ chunk is not a whole number of 4-line records',
+                   W.PARSE_HEADER: 'FASTQ record does not start with @',
+                   W.PARSE_FASTA_START: 'FASTA does not start with a > line',
+                   W.PARSE_FASTA_NAME: 'FASTA record with an empty name'}
+
+
+class QualityTooLong(ValueError):
+    """a FASTQ quality line is longer than its bases: the device layout keeps one quality per base at the bases' offsets, so
+    the chunk is parsed on the host instead (fastq.parse_fastq keeps such qualities as they are).  .index: the read."""
+
+    def __init__(self, index):
+        super().__init__('read %d has a quality line longer than its bases' % index)
+        self.index = index
+
+
+def initial_parse_caps(n_bytes, kind):
+    """(reads, name bytes, bases) of the first attempt of parse_reads for n_bytes of input: the bases fit in any case, names and
+    reads fit unless records average under 32 bytes; otherwise one more call with the exact counts"""
+    return n_bytes // 32 + 64, n_bytes // 4 + 4096, n_bytes
+
+
+def _kind_of(D, data, n):
+    """FASTQ or FASTA by the first byte, like fastq.parse_reads (get_sequence_file_type, misc.py:84-106)"""
+    head = bytes(D.host(D.head(data, 1))) if n else b''
+    if head == b'>':
+        return 'fasta'
+    if head in (b'@', b''):
+        return 'fastq'
+    raise ValueError('File is neither FASTA or FASTQ')
+
+
+def parse_reads(data, kind=None, qual=True):
+    """FASTQ / FASTA bytes in GPU memory -> the reads in GPU memory (pb200ParseReadsDevice): the fields fastq.parse_fastq /
+    fastq.parse_fasta return, field for field.  data: contiguous 1-D uint8 CUDA tensor of whole records; kind: 'fastq',
+    'fasta' or None (from the first byte, as fastq.parse_reads); qual=False writes no qualities (FASTA output).
+    Returns ParsedReads(names, name_off, seq, seq_off, qual, rna, kind) on the device -- the arguments trim_reads, demux_reads
+    and emit_reads take; qual is None when not asked for.  Malformed input raises the host parser's ValueError; a FASTQ quality
+    line longer than its bases raises QualityTooLong (with qual=True)."""
+    D = device()
+    if hasattr(D, 'check_bytes'):
+        D.check_bytes(data)
+    n = D.numel(data)
+    if kind is None:
+        kind = _kind_of(D, data, n)
+    if kind not in ('fastq', 'fasta'):
+        raise ValueError("kind must be 'fastq', 'fasta' or None")
+    reads_cap, names_cap, seq_cap = initial_parse_caps(n, kind)
+    for attempt in range(2):
+        names, seq = D.empty(max(names_cap, 1), np.uint8), D.empty(max(seq_cap, 1), np.uint8)
+        q = D.empty(max(seq_cap, 1), np.uint8) if qual else None
+        name_off, seq_off = D.empty(reads_cap + 1, np.int64), D.empty(reads_cap + 1, np.int64)
+        rna = D.empty(max(reads_cap, 1), np.uint8)
+        try:
+            n_reads, n_names, n_seq = W.pb200_parse_reads_device(
+                D.ptr(data), n, kind, d_names_ptr=D.ptr(names), names_cap=names_cap, d_name_off_ptr=D.ptr(name_off),
+                d_seq_ptr=D.ptr(seq), seq_cap=seq_cap, d_seq_off_ptr=D.ptr(seq_off), d_qual_ptr=D.ptr(q), d_rna_ptr=D.ptr(rna),
+                reads_cap=reads_cap, stream_ptr=D.stream())
+        except W.EngineError as e:
+            if e.code == W.ERR_SPACE and attempt == 0:
+                reads_cap, names_cap, seq_cap = e.n_reads, e.n_name_bytes, e.n_seq_bytes    # the exact counts: one more call
+                continue
+            reason = getattr(e, 'reason', 0)
+            if reason in _PARSE_MESSAGES:
+                raise ValueError(_PARSE_MESSAGES[reason]) from None
+            if reason == W.PARSE_LONG_QUAL:
+                raise QualityTooLong(e.index) from None
+            raise
+        break
+    return ParsedReads(D.head(names, n_names), D.head(name_off, n_reads + 1), D.head(seq, n_seq), D.head(seq_off, n_reads + 1),
+                       D.head(q, n_seq) if qual else None, D.head(rna, n_reads), kind)
+
+
+def _upload(D, data):
+    up = getattr(D, 'upload_bytes', None)
+    if up is not None:
+        return up(data)
+    return D.upload(np.frombuffer(data, dtype=np.uint8) if not isinstance(data, np.ndarray) else data)
+
+
+def _host_batch(data, kind):
+    if kind is None:
+        return fastq.parse_reads(data)[0]
+    return fastq.parse_fasta(data) if kind == 'fasta' else fastq.parse_fastq(data)
+
+
+def _device_chunk(data, kind, matching_sets, fmt, end_threshold, run):
+    """upload -> parse_reads -> run(parsed) -> emit_reads; None when the host path must take this chunk (a quality line longer
+    than its bases, no reads, nothing to align, or inputs the device call does not take: PB200_ERR_ARG)"""
+    if fmt not in ('fastq', 'fasta'):
+        raise ValueError("fmt must be 'fastq' or 'fasta'")
+    sets = fastq._norm_sets(matching_sets)
+    if end_threshold < 0 or not any(s or e for _, s, e in sets):
+        return None
+    D = device()
+    d_in = _upload(D, data)
+    try:
+        p = parse_reads(d_in, kind, qual=fmt == 'fastq')
+    except QualityTooLong:
+        return None
+    n = D.numel(p.rna)
+    if n == 0:
+        return None
+    try:
+        out = run(p, n)
+    except W.EngineError as e:
+        if e.code != W.ERR_ARG:
+            raise
+        return None
+    em = emit_reads(out, p.names, p.name_off, p.rna, fmt)
+    return out, em, getattr(D, 'download', D.host)(em.data), n
+
+
+def trim_fastq(data, matching_sets, scoring_scheme_vals, end_size=150, extra_end_trim=2, end_threshold=75.0, min_trim_size=4,
+               no_split=False, middle_threshold=85.0, extra_middle_trim_good_side=10, extra_middle_trim_bad_side=100,
+               min_split_read_size=1000, discard_middle=False, fmt='fastq', as_array=False, kind=None):
+    """fastq.trim_fastq on the device from input bytes to output bytes: host bytes of whole FASTQ / FASTA records (kind: 'fastq',
+    'fasta' or None = from the first byte) go up once, parse_reads -> trim_reads -> emit_reads run in GPU memory, and the output
+    bytes come home in one copy.  Returns (output bytes, or a uint8 array with as_array; info with start_trim, end_trim and
+    n_reads) -- the bytes fastq.trim_fastq writes for the parsed reads.  A chunk the device path does not take (a quality line
+    longer than its bases, inputs adapterTrimSplitReadsDevice refuses) runs through fastq.trim_fastq instead, with the same
+    result.  Malformed input raises the host parser's ValueError."""
+    opts = dict(end_size=end_size, extra_end_trim=extra_end_trim, end_threshold=end_threshold, min_trim_size=min_trim_size,
+                no_split=no_split, middle_threshold=middle_threshold, extra_middle_trim_good_side=extra_middle_trim_good_side,
+                extra_middle_trim_bad_side=extra_middle_trim_bad_side, min_split_read_size=min_split_read_size,
+                discard_middle=discard_middle)
+    got = _device_chunk(data, kind, matching_sets, fmt, end_threshold,
+                        lambda p, n: trim_reads(p.seq, p.seq_off, matching_sets, scoring_scheme_vals, p.qual, **opts))
+    if got is None:
+        return fastq.trim_fastq(_host_batch(data, kind), matching_sets, scoring_scheme_vals, fmt=fmt, as_array=as_array, **opts)
+    out, _, host, n = got
+    info = {'start_trim': np.asarray(out.start_trim, dtype=np.int64), 'end_trim': np.asarray(out.end_trim, dtype=np.int64),
+            'hits': out.hits, 'n_reads': n}
+    return (host if as_array else host.tobytes()), info
+
+
+def demux_fastq(data, matching_sets, scoring_scheme_vals, forward_or_reverse='forward', end_size=150, extra_end_trim=2,
+                end_threshold=75.0, min_trim_size=4, no_split=False, middle_threshold=85.0, extra_middle_trim_good_side=10,
+                extra_middle_trim_bad_side=100, min_split_read_size=1000, discard_middle=False, barcode_threshold=75.0,
+                barcode_diff=5.0, require_two_barcodes=False, discard_unassigned=False, untrimmed=False, fmt='fastq',
+                albacore_calls=None, as_array=False, kind=None):
+    """fastq.demux_fastq on the device from input bytes to output bytes, as trim_fastq: parse_reads -> demux_reads -> emit_reads,
+    and every bin's bytes are one slice of the single copy home.  albacore_calls: one bin name (or None) per read, one name for
+    every read, or None.  Returns ({bin name: bytes (or uint8 arrays with as_array)}, info with calls, start_trim, end_trim and
+    n_reads); chunks the device path does not take run through fastq.demux_fastq, with the same result."""
+    opts = dict(end_size=end_size, extra_end_trim=extra_end_trim, end_threshold=end_threshold, min_trim_size=min_trim_size,
+                no_split=no_split, middle_threshold=middle_threshold, extra_middle_trim_good_side=extra_middle_trim_good_side,
+                extra_middle_trim_bad_side=extra_middle_trim_bad_side, min_split_read_size=min_split_read_size,
+                discard_middle=discard_middle, untrimmed=untrimmed)
+    bc = dict(forward_or_reverse=forward_or_reverse, barcode_threshold=barcode_threshold, barcode_diff=barcode_diff,
+              require_two_barcodes=require_two_barcodes, discard_unassigned=discard_unassigned)
+
+    def calls_for(n):
+        return [albacore_calls] * n if isinstance(albacore_calls, str) else albacore_calls
+    got = _device_chunk(data, kind, matching_sets, fmt, end_threshold,
+                        lambda p, n: demux_reads(p.seq, p.seq_off, matching_sets, scoring_scheme_vals, p.qual,
+                                                 albacore_calls=calls_for(n), **bc, **opts))
+    if got is None:
+        batch = _host_batch(data, kind)
+        return fastq.demux_fastq(batch, matching_sets, scoring_scheme_vals, fmt=fmt, albacore_calls=calls_for(len(batch)),
+                                 as_array=as_array, **bc, **opts)
+    out, em, host, n = got
+    bins = {name: host[b0:b1] if as_array else host[b0:b1].tobytes() for name, (b0, b1) in em.bins.items()}
+    info = {'start_trim': np.asarray(out.start_trim, dtype=np.int64), 'end_trim': np.asarray(out.end_trim, dtype=np.int64),
+            'hits': out.hits, 'calls': out.calls, 'n_reads': n}
+    return bins, info

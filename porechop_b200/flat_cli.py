@@ -19,6 +19,10 @@ host rounds), PB200_CHECK_ALL_READS=1 runs Phase A over every read, and PB200_DE
 one best score per adapter sequence on the device (adapterSetSearch) -- what makes checking every read cheap.  With
 PB200_DEVICE_DECISIONS=1 and PB200_DEVICE_MIDDLE=1 both set, each chunk's Phase B and Phase C are one engine call
 (adapterTrimReads): the reads are uploaded once and the windows, trims and trimmed reads are made on the device.
+PB200_DEVICE_READS=1 takes each chunk from input bytes to output bytes on the device (device_reads.trim_fastq /
+demux_fastq): the raw bytes go up, are parsed there (pb200ParseReadsDevice), trimmed, split or demultiplexed and formatted
+there, and the output bytes come home in one copy; the background thread only reads (and gunzips) the input.  Chunks with
+nothing to align (no adapter set matched) and Phase A keep the host parse.
 
 Multi-GPU: launched with torchrun (one process per GPU) chunk c is handled by rank c % world on its own device; ranks
 write self-contained pieces and rank 0 stitches them in chunk order after a barrier -- no data-path collective
@@ -172,6 +176,9 @@ def main():
     chunk_bytes = int(os.environ.get('PB200_FLAT_CHUNK_BYTES', 256 << 20))
     # one process per GPU (torchrun): chunk c belongs to rank c % world; nothing but a final barrier is exchanged
     rank, world = int(os.environ.get('RANK', 0)), int(os.environ.get('WORLD_SIZE', 1))
+    device_reads = None
+    if os.environ.get('PB200_DEVICE_READS', '0') == '1':
+        from . import device_reads
     if world > 1:
         import torch.distributed as dist
         from . import cpp_function_wrappers as W
@@ -180,6 +187,9 @@ def main():
         n_dev = W.device_count()
         if n_dev > 0:
             W.set_device(int(os.environ.get('LOCAL_RANK', rank)) % n_dev)
+            if device_reads is not None:        # device_reads allocates on torch's current device: the engine's
+                import torch
+                torch.cuda.set_device(int(os.environ.get('LOCAL_RANK', rank)) % n_dev)
         dist.init_process_group('gloo')                   # host-side barrier only; the data path has no collective
         local_world = int(os.environ.get('LOCAL_WORLD_SIZE', world))
         hostio.set_threads(max(1, hostio.usable_cpus() // max(local_world, 1)))    # torchrun exports OMP_NUM_THREADS=1
@@ -259,19 +269,29 @@ def main():
         os.makedirs(args.barcode_dir, exist_ok=True)
 
     def process(batch, albacore_call, chunk):
+        # batch: a FastqBatch, or with PB200_DEVICE_READS=1 (kind, raw bytes) -- parsed on the host only when nothing is aligned
+        on_device = device_reads is not None and sets
+        if device_reads is not None and not sets:
+            batch = parsers[batch[0]](batch[1])
         if args.barcode_dir is None:
-            if sets:
+            if on_device:
+                out, _ = device_reads.trim_fastq(batch[1], sets, scoring, kind=batch[0], **common)
+            elif sets:
                 out, _ = fastq.trim_fastq(batch, sets, scoring, **common)
             else:                   # "No adapters found - output reads are unchanged from input reads"
                 out = fastq.emit(batch, fmt=fmt, as_array=True)
             sink(None).write(out, chunk)
             return
         if sets:
-            calls = None if albacore_call is None else [albacore_call] * len(batch)
-            bins, _ = fastq.demux_fastq(batch, sets, scoring, direction, barcode_threshold=args.barcode_threshold,
-                                        barcode_diff=args.barcode_diff, require_two_barcodes=args.require_two_barcodes,
-                                        discard_unassigned=args.discard_unassigned, untrimmed=args.untrimmed,
-                                        albacore_calls=calls, **common)
+            bc = dict(barcode_threshold=args.barcode_threshold, barcode_diff=args.barcode_diff,
+                      require_two_barcodes=args.require_two_barcodes, discard_unassigned=args.discard_unassigned,
+                      untrimmed=args.untrimmed)
+            if on_device:
+                bins, _ = device_reads.demux_fastq(batch[1], sets, scoring, direction, albacore_calls=albacore_call,
+                                                   kind=batch[0], **bc, **common)
+            else:
+                calls = None if albacore_call is None else [albacore_call] * len(batch)
+                bins, _ = fastq.demux_fastq(batch, sets, scoring, direction, albacore_calls=calls, **bc, **common)
         else:
             out = fastq.emit(batch, fmt=fmt, untrimmed=args.untrimmed, as_array=True)
             bins = {} if args.discard_unassigned else {'none': out}
@@ -283,7 +303,7 @@ def main():
         for path, albacore_call in zip(inputs, albacore):
             for kind, data in _record_chunks(path, chunk_bytes, 0):
                 if chunk % world == rank:
-                    yield parsers[kind](data), albacore_call, chunk
+                    yield ((kind, data) if device_reads is not None else parsers[kind](data)), albacore_call, chunk
                 chunk += 1
     for batch, albacore_call, chunk in _prefetch(batches()):
         process(batch, albacore_call, chunk)

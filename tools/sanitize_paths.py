@@ -128,6 +128,13 @@ def split_reads():
         if em.data.cpu().numpy().tobytes() != fastq.emit_parts(names, name_off, rna, parts if fmt == 'fastq' else
                                                                (parts[0], None) + parts[2:], fmt):
             return np.zeros(1), np.ones(1)
+    # the reads' FASTQ / FASTA bytes parsed on the device (pb200ParseReadsDevice): the host parser's fields
+    text = fastq.emit(fastq.FastqBatch(names, name_off, lbuf, loff, qual, loff, rna), fmt='fastq')
+    for kind, data in (('fastq', text), ('fasta', fastq.emit(fastq.parse_fastq(text), fmt='fasta'))):
+        p = device_reads.parse_reads(torch.from_numpy(np.frombuffer(data, dtype=np.uint8).copy()).cuda(), kind)
+        hb = fastq.parse_fastq(data) if kind == 'fastq' else fastq.parse_fasta(data)
+        if any(not np.array_equal(x.cpu().numpy(), y) for x, y in zip(p[:5], (hb.name_buf, hb.name_off, hb.seq, hb.seq_off, hb.qual))):
+            return np.zeros(1), np.ones(1)
     st, et, _, _, n_hits, h = W.adapter_trim_reads(lbuf, loff, sides[0], sides[1], (a2, o2), wl.DEFAULT_SCORING, 150, 2, 75.0, 4, 85.0)
     middle = fastq.middle_trim_ranges(fastq._hits_dict(n_hits, h), [('t', yt), ('b', yb)], {'t'}, {'b'}, 10, 100)
     batch = fastq.FastqBatch(names, name_off, lbuf, loff, qual, loff, rna)
