@@ -358,6 +358,33 @@ typedef struct {
     int64_t *error_index;              /* host out: first bad record (FASTQ) or line (FASTA), -1 when none                    */
 } pb200_parse_args_t;
 int pb200ParseReadsDevice(const pb200_parse_args_t *args, void *stream);
+/* gzip (RFC 1952) of bytes in device memory, e.g. pb200EmitReadsDevice's output, into a caller-owned device buffer.  The input
+ * is partitioned into segments (files, or a demux's bins): seg_off[0] = 0 <= seg_off[1] <= ... <= seg_off[n_segs] = n.  Each
+ * segment is cut into blocks of `block` bytes (the last one shorter), and every block becomes one gzip member: the 10-byte
+ * header 1f 8b 08 00 00 00 00 00 00 03, one dynamic-Huffman deflate block (RFC 1951; LZ77 matches inside the block, codes
+ * built from the block's own symbols) or, when that would not be smaller, stored blocks, then CRC-32 and ISIZE.  Segment s's
+ * members are d_out[out_seg_off[s] .. out_seg_off[s + 1]): a file whose decompression is the segment's bytes.  An empty
+ * segment gets no bytes.  The output depends on the input, seg_off and block alone (the same bytes on every run and GPU).
+ * *n_out_bytes and out_seg_off are always written; if the total exceeds out_cap the call returns PB200_ERR_SPACE and d_out is
+ * not written.  pb200GzipBound(n, n_segs, block) is never less than the total.  The call returns once the device output is
+ * written; stream and ordering rules as pb200EmitReadsDevice.
+ * Preconditions, checked before the device is touched (PB200_ERR_ARG otherwise): args, seg_off, out_seg_off and n_out_bytes
+ * not NULL; n >= 0, n_segs >= 1, out_cap >= 0; seg_off ascending from 0 to n; block 0 (the default, 65536) or 4096 .. 131072;
+ * d_src when n > 0 and d_out when out_cap > 0. */
+typedef struct {
+    const uint8_t *d_src;              /* device, n bytes                                                                     */
+    int64_t n;
+    const int64_t *seg_off;            /* host, n_segs + 1                                                                    */
+    int64_t n_segs;
+    int32_t block;                     /* bytes per member (0: 65536)                                                         */
+    uint8_t *d_out;                    /* device, out_cap bytes                                                               */
+    int64_t out_cap;
+    int64_t *out_seg_off;              /* host out, n_segs + 1: the segments' byte ranges in d_out                            */
+    int64_t *n_out_bytes;              /* host out, always written                                                            */
+} pb200_gzip_args_t;
+int pb200GzipDevice(const pb200_gzip_args_t *args, void *stream);
+/* The most bytes pb200GzipDevice writes for n bytes in n_segs segments (every block stored), or -1 for arguments it refuses. */
+int64_t pb200GzipBound(int64_t n, int64_t n_segs, int32_t block);
 /* cmin[l], l = 0 .. len-1: the smallest c with float("%f" % (100.0*c/l)) >= middle_threshold, or l+1 if none does
  * (cmin[0] = INT32_MAX).  The ">=" sibling of pb200TrimThresholdTable.  Pure host code; middle_threshold must be > 0. */
 int pb200MiddleThresholdTable(double middle_threshold, int32_t len, int32_t *cmin);

@@ -147,6 +147,18 @@ class ParseArgsDesc(Structure):
 
 C_LIB.pb200ParseReadsDevice.argtypes = [POINTER(ParseArgsDesc), c_void_p]
 C_LIB.pb200ParseReadsDevice.restype = c_int
+
+
+class GzipArgsDesc(Structure):
+    """pb200_gzip_args_t (include/porechop_b200.h)"""
+    _fields_ = [('d_src', c_void_p), ('n', c_int64), ('seg_off', c_void_p), ('n_segs', c_int64), ('block', c_int32),
+                ('d_out', c_void_p), ('out_cap', c_int64), ('out_seg_off', c_void_p), ('n_out_bytes', c_void_p)]
+
+
+C_LIB.pb200GzipDevice.argtypes = [POINTER(GzipArgsDesc), c_void_p]
+C_LIB.pb200GzipDevice.restype = c_int
+C_LIB.pb200GzipBound.argtypes = [c_int64, c_int64, c_int32]
+C_LIB.pb200GzipBound.restype = c_int64
 C_LIB.pb200MiddleThresholdTable.argtypes = [c_double, c_int32, c_void_p]
 C_LIB.pb200MiddleThresholdTable.restype = c_int
 C_LIB.pb200FormatRecord.argtypes = [c_void_p, c_char_p, c_int]
@@ -172,7 +184,7 @@ EXPORTED_SYMBOLS = ['adapterAlignment', 'freeCString', 'adapterAlignmentBatch', 
                     'adapterAlignmentBatchDevice', 'adapterEndDecisions', 'pb200TrimThresholdTable', 'adapterSetSearch',
                     'adapterMiddleScan',
                     'adapterMiddleScanDevice', 'pb200MiddleThresholdTable', 'adapterTrimReads', 'adapterTrimReadsDevice',
-                    'adapterTrimSplitReadsDevice', 'adapterDemuxReadsDevice', 'pb200EmitReadsDevice', 'pb200ParseReadsDevice', 'pb200FormatRecord', 'pb200DeviceCount', 'pb200SetDevice', 'pb200Synchronize', 'pb200LastError',
+                    'adapterTrimSplitReadsDevice', 'adapterDemuxReadsDevice', 'pb200EmitReadsDevice', 'pb200ParseReadsDevice', 'pb200GzipDevice', 'pb200GzipBound', 'pb200FormatRecord', 'pb200DeviceCount', 'pb200SetDevice', 'pb200Synchronize', 'pb200LastError',
                     'pb200KernelLaunches', 'pb200TimingEnable', 'pb200TimingRead', 'pb200TimingReadKinds', 'pb200SetOption',
                     'pb200GetOption', 'pb200HostBuffer', 'pb200PackNibbles']
 
@@ -633,6 +645,32 @@ def pb200_parse_reads_device(d_in_ptr, n_in, fmt='fastq', *, d_names_ptr=0, name
         e.reason, e.index = err.value, err_index.value
         raise
     return tuple(x.value for x in outs)
+
+
+def gzip_bound(n, n_segs=1, block=0):
+    """the most bytes pb200_gzip_device writes for n bytes in n_segs segments with this block size (pb200GzipBound)"""
+    b = C_LIB.pb200GzipBound(int(n), int(n_segs), int(block))
+    if b < 0:
+        raise ValueError('n must be >= 0, n_segs >= 1 and block 0 or 4096 .. 131072')
+    return b
+
+
+def pb200_gzip_device(d_src_ptr, n, seg_off=None, *, block=0, d_out_ptr=0, out_cap=0, stream_ptr=0):
+    """gzip members of n bytes in device memory (pb200GzipDevice) into d_out (out_cap bytes): seg_off (int64[n_segs + 1],
+    ascending from 0 to n; None = one segment) partitions the input into files, each cut into members of `block` bytes
+    (0 = the default).  Returns (total bytes, int64 array of the segments' byte offsets in d_out).  When they do not fit
+    out_cap it raises EngineError with code ERR_SPACE, the total as .n_out_bytes and the offsets as .out_seg_off."""
+    seg = np.ascontiguousarray(np.array([0, n] if seg_off is None else seg_off, dtype=np.int64))
+    out_off = np.zeros(max(len(seg), 1), dtype=np.int64)
+    n_out = c_int64(0)
+    args = GzipArgsDesc(d_src_ptr or None, int(n), _ptr(seg), len(seg) - 1, int(block), d_out_ptr or None, int(out_cap),
+                        _ptr(out_off), addressof(n_out))
+    try:
+        _check(C_LIB.pb200GzipDevice(byref(args), c_void_p(stream_ptr)))
+    except EngineError as e:
+        e.n_out_bytes, e.out_seg_off = n_out.value, out_off
+        raise
+    return n_out.value, out_off
 
 
 def middle_threshold_table(middle_threshold, length):

@@ -758,4 +758,230 @@ PB_HD int32_t barcode_call(const BarcodeSide &s, const BarcodeSide &e, int32_t n
     return call;
 }
 
+// ---- gzip members (pb200GzipDevice): the parts of the deflate encoder (RFC 1951) that need no CUDA ---------------------------
+// gzip_block_kernel (kernels.cuh) runs them on the device and tests/emu/emu_gzip.cpp on the host.
+constexpr int GZ_LITLEN = 286;          // literal / length symbols 0..285 (256 = end of block)
+constexpr int GZ_DIST = 30;             // distance symbols
+constexpr int GZ_CL = 19;               // code-length symbols
+constexpr int GZ_MAX_BITS = 15;         // limit of the literal / length and distance codes
+constexpr int GZ_CL_MAX_BITS = 7;       // limit of the code-length code
+constexpr int GZ_HEADER = 10;           // member header 1f 8b 08 00 00000000 00 03 (what zlib writes at level 6)
+constexpr int GZ_TRAILER = 8;           // CRC-32 and ISIZE
+constexpr int GZ_STORED_MAX = 65535;    // bytes of one stored block
+
+PB_HD int gz_log2(uint32_t x) {         // floor(log2(x)), x > 0
+#if defined(__CUDA_ARCH__)
+    return 31 - __clz(x);
+#else
+    return 31 - __builtin_clz(x);
+#endif
+}
+// match length 3..258 -> symbol 257..285, its extra bits and their value
+PB_HD void gz_len_sym(int len, int &sym, int &nextra, int &extra) {
+    if (len == 258) { sym = 285; nextra = 0; extra = 0; return; }
+    const int l = len - 3;
+    if (l < 8) { sym = 257 + l; nextra = 0; extra = 0; return; }
+    const int e = gz_log2((uint32_t)l) - 2;
+    sym = 257 + 4 * (e + 1) + ((l >> e) - 4);
+    nextra = e;
+    extra = l & ((1 << e) - 1);
+}
+// distance 1..32768 -> symbol 0..29, its extra bits and their value
+PB_HD void gz_dist_sym(int dist, int &sym, int &nextra, int &extra) {
+    const int x = dist - 1;
+    if (x < 4) { sym = x; nextra = 0; extra = 0; return; }
+    const int e = gz_log2((uint32_t)x) - 1;
+    sym = 2 * e + ((x >> e) & 1) + 2;
+    nextra = e;
+    extra = x & ((1 << e) - 1);
+}
+PB_HD int gz_len_extra_bits(int sym) { return sym < 265 || sym == 285 ? 0 : (sym - 261) / 4; }
+PB_HD int gz_dist_extra_bits(int sym) { return sym < 4 ? 0 : sym / 2 - 1; }
+
+// Length-limited Huffman code lengths of freq[0 .. n) (n <= 512): len[s] = 0 for an unused symbol, else 1..limit.  At least two
+// symbols get a code (the first unused ones are added when fewer are used): inflate refuses an incomplete code-length code, and
+// a one-code tree needs the same care.  Minimum-redundancy lengths by Moffat and Katajainen's in-place method on the symbols
+// sorted by (frequency, symbol); lengths over the limit are cut to it and the Kraft sum is repaired by lengthening the
+// deepest codes that still fit (the heuristic miniz and others use).  work: 2n + 16 words.
+PB_HD void gz_code_lengths(const uint32_t *freq, int n, int limit, uint8_t *len, uint32_t *work) {
+    uint32_t *key = work, *A = work + n, *count = work + 2 * n;
+    int m = 0;
+    for (int s = 0; s < n; ++s) {
+        len[s] = 0;
+        if (freq[s]) key[m++] = (freq[s] << 9) | (uint32_t)s;
+    }
+    for (int s = 0; s < n && m < 2; ++s)
+        if (!freq[s]) key[m++] = (1u << 9) | (uint32_t)s;
+    for (int i = 1; i < m; ++i) {                                // insertion sort: m <= 286
+        const uint32_t k = key[i];
+        int j = i - 1;
+        while (j >= 0 && key[j] > k) { key[j + 1] = key[j]; --j; }
+        key[j + 1] = k;
+    }
+    for (int i = 0; i < m; ++i) A[i] = key[i] >> 9;
+    // first pass: parents; second: internal depths; third: leaf depths (A[i] = depth of the i-th least frequent symbol)
+    A[0] += A[1];
+    int root = 0, leaf = 2;
+    for (int next = 1; next < m - 1; ++next) {
+        if (leaf >= m || A[root] < A[leaf]) { A[next] = A[root]; A[root++] = (uint32_t)next; }
+        else A[next] = A[leaf++];
+        if (leaf >= m || (root < next && A[root] < A[leaf])) { A[next] += A[root]; A[root++] = (uint32_t)next; }
+        else A[next] += A[leaf++];
+    }
+    A[m - 2] = 0;
+    for (int next = m - 3; next >= 0; --next) A[next] = A[A[next]] + 1;
+    int avail = 1, used = 0, depth = 0, next = m - 1;
+    root = m - 2;
+    while (avail > 0) {
+        while (root >= 0 && (int)A[root] == depth) { ++used; --root; }
+        while (avail > used) { A[next--] = (uint32_t)depth; --avail; }
+        avail = 2 * used; ++depth; used = 0;
+    }
+    for (int l = 0; l <= limit; ++l) count[l] = 0;
+    for (int i = 0; i < m; ++i) count[A[i] < (uint32_t)limit ? A[i] : (uint32_t)limit]++;
+    uint32_t kraft = 0;                                          // in units of 2^-limit
+    for (int l = 1; l <= limit; ++l) kraft += count[l] << (limit - l);
+    while (kraft > (1u << limit)) {
+        count[limit]--;
+        for (int l = limit - 1; l > 0; --l)
+            if (count[l]) { count[l]--; count[l + 1] += 2; break; }
+        kraft--;
+    }
+    int i = 0;                                                   // least frequent symbols get the longest codes
+    for (int l = limit; l >= 1; --l)
+        for (uint32_t c = 0; c < count[l]; ++c) len[key[i++] & 511u] = (uint8_t)l;
+}
+// canonical codes of len[0 .. n), bit-reversed (deflate sends Huffman codes from their first bit, the bit packer from bit 0)
+PB_HD void gz_canonical_codes(const uint8_t *len, int n, uint16_t *code) {
+    uint32_t next[GZ_MAX_BITS + 2];
+    for (int l = 0; l <= GZ_MAX_BITS + 1; ++l) next[l] = 0;
+    for (int s = 0; s < n; ++s) next[len[s] + 1]++;
+    next[1] = 0;                                                 // count[0] (unused symbols) starts no code
+    for (int l = 1; l <= GZ_MAX_BITS; ++l) next[l + 1] = (next[l] + next[l + 1]) << 1;
+    for (int s = 0; s < n; ++s) {
+        const int l = len[s];
+        if (!l) { code[s] = 0; continue; }
+        uint32_t c = next[l]++, r = 0;
+        for (int b = 0; b < l; ++b) { r = (r << 1) | (c & 1u); c >>= 1; }
+        code[s] = (uint16_t)r;
+    }
+}
+
+// The code-length sequence of a dynamic block: HLIT + HDIST lengths, run-length coded with 16 (repeat the previous length
+// 3-6 times, 2 extra bits), 17 (3-10 zeros, 3 bits) and 18 (11-138 zeros, 7 bits).  Returns the number of symbols.
+PB_HD int gz_rle(const uint8_t *lens, int total, uint8_t *sym, uint8_t *extra) {
+    int k = 0, i = 0;
+    while (i < total) {
+        const uint8_t v = lens[i];
+        int run = 1;
+        while (i + run < total && lens[i + run] == v) ++run;
+        i += run;
+        if (v == 0) {
+            while (run >= 11) { const int r = run < 138 ? run : 138; sym[k] = 18; extra[k++] = (uint8_t)(r - 11); run -= r; }
+            if (run >= 3) { sym[k] = 17; extra[k++] = (uint8_t)(run - 3); run = 0; }
+        } else {
+            sym[k] = v; extra[k++] = 0; --run;
+            while (run >= 3) { const int r = run < 6 ? run : 6; sym[k] = 16; extra[k++] = (uint8_t)(r - 3); run -= r; }
+        }
+        while (run-- > 0) { sym[k] = v; extra[k++] = 0; }
+    }
+    return k;
+}
+PB_HD int gz_cl_extra_bits(int sym) { return sym == 16 ? 2 : sym == 17 ? 3 : sym == 18 ? 7 : 0; }
+// the order in which the code-length code's lengths are sent
+PB_HD int gz_cl_order(int i) {
+    const uint8_t order[GZ_CL] = {16, 17, 18, 0, 8, 7, 9, 6, 10, 5, 11, 4, 12, 3, 13, 2, 14, 1, 15};
+    return order[i];
+}
+
+// LSB-first bits into zeroed 32-bit words (one writer)
+struct GzBitWriter {
+    uint32_t *w;
+    uint64_t pos;
+    PB_HD void put(uint32_t bits, int n) {                       // n <= 32, bits < 2^n
+        if (!n) return;
+        const int sh = (int)(pos & 31);
+        w[pos >> 5] |= bits << sh;
+        if (sh + n > 32) w[(pos >> 5) + 1] |= bits >> (32 - sh);
+        pos += (uint64_t)n;
+    }
+};
+
+// Everything a dynamic block's header needs, from the literal / length and distance lengths
+struct GzDynHeader {
+    int hlit, hdist, hclen, n_rle;
+    uint8_t rle_sym[GZ_LITLEN + GZ_DIST], rle_extra[GZ_LITLEN + GZ_DIST];
+    uint8_t cl_len[GZ_CL];
+    uint16_t cl_code[GZ_CL];
+};
+// fills H and returns the header's bits (block header included); all_lens: scratch of GZ_LITLEN + GZ_DIST bytes; work as
+// gz_code_lengths
+PB_HD uint64_t gz_dynamic_header(const uint8_t *ll_len, const uint8_t *d_len, GzDynHeader &H, uint8_t *all_lens, uint32_t *work) {
+    H.hlit = GZ_LITLEN;
+    while (H.hlit > 257 && !ll_len[H.hlit - 1]) --H.hlit;
+    H.hdist = GZ_DIST;
+    while (H.hdist > 1 && !d_len[H.hdist - 1]) --H.hdist;
+    for (int s = 0; s < H.hlit; ++s) all_lens[s] = ll_len[s];
+    for (int s = 0; s < H.hdist; ++s) all_lens[H.hlit + s] = d_len[s];
+    H.n_rle = gz_rle(all_lens, H.hlit + H.hdist, H.rle_sym, H.rle_extra);
+    uint32_t cl_freq[GZ_CL];
+    for (int s = 0; s < GZ_CL; ++s) cl_freq[s] = 0;
+    for (int k = 0; k < H.n_rle; ++k) cl_freq[H.rle_sym[k]]++;
+    gz_code_lengths(cl_freq, GZ_CL, GZ_CL_MAX_BITS, H.cl_len, work);
+    gz_canonical_codes(H.cl_len, GZ_CL, H.cl_code);
+    H.hclen = GZ_CL;
+    while (H.hclen > 4 && !H.cl_len[gz_cl_order(H.hclen - 1)]) --H.hclen;
+    uint64_t bits = 3 + 5 + 5 + 4 + 3 * (uint64_t)H.hclen;
+    for (int k = 0; k < H.n_rle; ++k) bits += (uint64_t)(H.cl_len[H.rle_sym[k]] + gz_cl_extra_bits(H.rle_sym[k]));
+    return bits;
+}
+PB_HD void gz_write_dynamic_header(GzBitWriter &bw, int bfinal, const GzDynHeader &H) {
+    bw.put((uint32_t)bfinal | (2u << 1), 3);
+    bw.put((uint32_t)(H.hlit - 257), 5);
+    bw.put((uint32_t)(H.hdist - 1), 5);
+    bw.put((uint32_t)(H.hclen - 4), 4);
+    for (int i = 0; i < H.hclen; ++i) bw.put(H.cl_len[gz_cl_order(i)], 3);
+    for (int k = 0; k < H.n_rle; ++k) {
+        const int s = H.rle_sym[k];
+        bw.put(H.cl_code[s], H.cl_len[s]);
+        bw.put(H.rle_extra[k], gz_cl_extra_bits(s));
+    }
+}
+// bytes of n input bytes as stored blocks (each: 3 header bits padded to a byte, LEN, NLEN, the bytes)
+PB_HD int64_t gz_stored_bytes(int64_t n) { return n + 5 * ((n + GZ_STORED_MAX - 1) / GZ_STORED_MAX); }
+// the largest member of a block of `block` bytes: header, stored blocks, trailer
+PB_HD int64_t gz_member_bound(int64_t block) { return GZ_HEADER + gz_stored_bytes(block) + GZ_TRAILER; }
+
+// ---- CRC-32 (the gzip trailer): table-driven, and the CRC of a concatenation from the CRCs of its parts ----
+constexpr uint32_t GZ_CRC_POLY = 0xEDB88320u;                    // reflected x^32 + x^26 + ... + 1
+PB_HD uint32_t gz_crc_table_entry(uint32_t i) {
+    uint32_t c = i;
+    for (int k = 0; k < 8; ++k) c = (c & 1u) ? (c >> 1) ^ GZ_CRC_POLY : c >> 1;
+    return c;
+}
+// CRC-32 of p[0 .. n) continuing from crc (0 for the first bytes), with a 256-entry table
+PB_HD uint32_t gz_crc_update(uint32_t crc, const uint32_t *table, const uint8_t *p, int64_t n) {
+    crc = ~crc;
+    for (int64_t i = 0; i < n; ++i) crc = table[(crc ^ p[i]) & 0xFFu] ^ (crc >> 8);
+    return ~crc;
+}
+// a * b modulo the CRC polynomial, both in the reflected representation (bit 31 = x^0)
+PB_HD uint32_t gz_crc_mulmod(uint32_t a, uint32_t b) {
+    uint32_t p = 0;
+    for (uint32_t m = 1u << 31; m; m >>= 1) {
+        if (a & m) p ^= b;
+        b = (b & 1u) ? (b >> 1) ^ GZ_CRC_POLY : b >> 1;
+    }
+    return p;
+}
+// CRC-32 of A || B from crc_a, crc_b and the length of B: crc_a times x^(8 len_b), plus crc_b
+PB_HD uint32_t gz_crc_combine(uint32_t crc_a, uint32_t crc_b, int64_t len_b) {
+    uint32_t p = 1u << 31, q = 1u << 23;                         // x^0, x^8
+    for (uint64_t n = (uint64_t)len_b; n; n >>= 1) {
+        if (n & 1u) p = gz_crc_mulmod(q, p);
+        q = gz_crc_mulmod(q, q);
+    }
+    return gz_crc_mulmod(p, crc_a) ^ crc_b;
+}
+
 }  // namespace pb

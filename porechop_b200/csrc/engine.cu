@@ -209,7 +209,10 @@ struct Engine {
     // parse (pb200ParseReadsDevice): line counts per tile (scanned), line ends, the per-record (FASTQ) or per-line (FASTA) index
     // arrays, and one status byte per record or line
     DevBuf parse_tiles, parse_lines, parse_index, parse_status;
-    std::shared_ptr<void> packer;        // Packer (below): the thread that plans and packs chunks ahead of the submit loop
+    // gzip (pb200GzipDevice): the block table (source offsets, lengths, slot offsets), one member slot and one token buffer per
+    // block, the members' sizes (scanned into their offsets)
+    DevBuf gz_table, gz_slots, gz_tokens, gz_sizes;
+    std::shared_ptr<void> packer;       // Packer (below): the thread that plans and packs chunks ahead of the submit loop
     // Ordering between calls: every entry point uses the stage buffers above (st[0]'s trace scratch, tasks, codes, status word),
     // whatever stream it runs on.  A call that returns with work still queued (adapterAlignmentBatchDevice) records `last` on
     // its stream; every later call's streams wait for it before they touch a buffer (order_after_last).  `last_pending` is
@@ -2593,6 +2596,86 @@ int parse_reads(const pb200_parse_args_t *A, void *user_stream) {
     });
 }
 
+// ---- gzip members (pb200GzipDevice) ------------------------------------------------------------------------------------
+int64_t gzip_block_of(int32_t block) { return block == 0 ? PB_GZ_DEFAULT_BLOCK : block; }
+// most bytes for n bytes in n_segs segments: every member stored; a segment adds at most one short block
+int64_t gzip_bound(int64_t n, int64_t n_segs, int64_t block) {
+    const int64_t members = n == 0 ? 0 : (n + block - 1) / block + n_segs - 1;
+    return n + members * (gz_member_bound(block) - block);
+}
+// The block table goes up, one CTA per block writes its member into its slot, the sizes are scanned into offsets and come home
+// with the status word in one synchronise; then, when the total fits, split_gather_kernel packs the members into d_out.
+int gzip_device(const pb200_gzip_args_t *A, void *user_stream) {
+    if (!A) return fail(PB200_ERR_ARG, "NULL pointer");
+    if (A->n_out_bytes) *A->n_out_bytes = 0;
+    if (!A->n_out_bytes || !A->seg_off || !A->out_seg_off) return fail(PB200_ERR_ARG, "NULL pointer");
+    if (A->n < 0 || A->n_segs < 1 || A->out_cap < 0) return fail(PB200_ERR_ARG, "negative count (or no segment)");
+    if ((A->n > 0 && !A->d_src) || (A->out_cap > 0 && !A->d_out)) return fail(PB200_ERR_ARG, "NULL pointer");
+    if (A->block != 0 && (A->block < PB_GZ_MIN_BLOCK || A->block > PB_GZ_MAX_BLOCK))
+        return fail(PB200_ERR_ARG, "block must be 0 (default) or 4096 .. 131072");
+    const int64_t ns = A->n_segs, n = A->n;
+    if (A->seg_off[0] != 0 || A->seg_off[ns] != n) return fail(PB200_ERR_ARG, "seg_off must run from 0 to n");
+    for (int64_t s = 0; s < ns; ++s)
+        if (A->seg_off[s + 1] < A->seg_off[s]) return fail(PB200_ERR_ARG, "seg_off is not ascending");
+    const int32_t block = (int32_t)gzip_block_of(A->block);
+    const int64_t stride = (gz_member_bound(block) + 15) & ~(int64_t)15;
+    std::vector<int64_t> start, len, first(ns + 1);        // blocks; the first block of every segment
+    for (int64_t s = 0; s < ns; ++s) {
+        first[s] = (int64_t)start.size();
+        for (int64_t p = A->seg_off[s]; p < A->seg_off[s + 1]; p += block) {
+            start.push_back(p);
+            len.push_back(std::min<int64_t>(block, A->seg_off[s + 1] - p));
+        }
+    }
+    const int64_t nb = (int64_t)start.size();
+    first[ns] = nb;
+    std::vector<int64_t> table(3 * nb);
+    for (int64_t b = 0; b < nb; ++b) { table[b] = start[b]; table[nb + b] = len[b]; table[2 * nb + b] = b * stride; }
+    return sync_call(CallOn::library, user_stream, [&](Engine &E, cudaStream_t stream) -> int {
+        NvtxRange range("pb200:gzip");
+        Stage &S = E.st[0];
+        if (int rc = reset_misc(S, stream)) return rc;
+        std::vector<int64_t> off(nb + 1, 0);
+        int st = 0;
+        if (nb > 0) {
+            if (int rc = E.gz_table.ensure((size_t)nb * 24)) return rc;
+            if (int rc = E.gz_slots.ensure((size_t)(nb * stride))) return rc;
+            if (int rc = E.gz_tokens.ensure((size_t)nb * block * 4)) return rc;
+            if (int rc = E.gz_sizes.ensure((size_t)(nb + 1) * 8)) return rc;
+            int64_t *tab = E.gz_table.as<int64_t>(), *sizes = E.gz_sizes.as<int64_t>();
+            CK(cudaMemcpyAsync(tab, table.data(), (size_t)nb * 24, cudaMemcpyHostToDevice, stream));
+            const size_t smem = (size_t)gz_smem_bytes(block);
+            int bps = 0;
+            if (int rc = E.blocks_per_sm(reinterpret_cast<const void *>(&gzip_block_kernel), PB_GZ_THREADS, smem, &bps)) return rc;
+            gzip_block_kernel<<<(unsigned)nb, PB_GZ_THREADS, smem, stream>>>(A->d_src, static_cast<const int64_t *>(tab),
+                                                                            static_cast<const int64_t *>(tab + nb), block,
+                                                                            E.gz_slots.as<uint8_t>(), stride,
+                                                                            E.gz_tokens.as<uint32_t>(), sizes);
+            g_launches++;
+            CK(cudaGetLastError());
+            if (int rc = scan_offsets(E, stream, sizes, nb)) return rc;
+            CK(cudaMemcpyAsync(off.data(), sizes, (size_t)(nb + 1) * 8, cudaMemcpyDeviceToHost, stream));
+        }
+        CK(cudaMemcpyAsync(&st, S.misc.p, 4, cudaMemcpyDeviceToHost, stream));
+        CK(cudaStreamSynchronize(stream));
+        for (int64_t s = 0; s <= ns; ++s) A->out_seg_off[s] = off[first[s]];
+        *A->n_out_bytes = off[nb];
+        if (int rc = status_error(st)) return rc;          // a deferred error of an earlier device-resident call
+        if (off[nb] > A->out_cap) return fail(PB200_ERR_SPACE, "out_cap is smaller than the output (*n_out_bytes)");
+        if (nb > 0) {
+            const int64_t blocks = std::max<int64_t>(1, std::min<int64_t>((nb + 7) / 8, (int64_t)E.sm_count * 8));
+            split_gather_kernel<<<(unsigned)blocks, 256, 0, stream>>>(E.gz_slots.as<uint8_t>(), nullptr,
+                                                                      static_cast<const int64_t *>(E.gz_table.as<int64_t>() + 2 * nb),
+                                                                      static_cast<const int64_t *>(E.gz_sizes.as<int64_t>()), nb,
+                                                                      A->d_out, nullptr);
+            g_launches++;
+            CK(cudaGetLastError());
+            CK(cudaStreamSynchronize(stream));              // the device output is written when the call returns
+        }
+        return 0;
+    });
+}
+
 }  // namespace
 
 // =====================================================================================================
@@ -2684,6 +2767,16 @@ int pb200EmitReadsDevice(const pb200_emit_args_t *args, int64_t n_rec, void *str
 int pb200ParseReadsDevice(const pb200_parse_args_t *args, void *stream) {
     g_err.clear();
     return parse_reads(args, stream);
+}
+
+int pb200GzipDevice(const pb200_gzip_args_t *args, void *stream) {
+    g_err.clear();
+    return gzip_device(args, stream);
+}
+
+int64_t pb200GzipBound(int64_t n, int64_t n_segs, int32_t block) {
+    if (n < 0 || n_segs < 1 || (block != 0 && (block < PB_GZ_MIN_BLOCK || block > PB_GZ_MAX_BLOCK))) return -1;
+    return gzip_bound(n, n_segs, gzip_block_of(block));
 }
 
 int pb200MiddleThresholdTable(double middle_threshold, int32_t len, int32_t *cmin) {

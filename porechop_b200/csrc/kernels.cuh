@@ -1693,6 +1693,238 @@ __global__ void __launch_bounds__(PB_DEMUX_TILE) demux_scatter_kernel(const int3
 }
 
 // ---------------------------------------------------------------------------------------------------
+// pb200GzipDevice: one gzip member per block of input (a block never crosses a segment), one CTA per block, written into a
+// fixed slot of engine scratch.  The CTA stages the block in shared memory and
+//   1. takes the CRC-32 of 256 slices (one per thread) and combines them in a tree;
+//   2. finds matches in rounds of one position per thread: the most recent earlier position with the same 3-byte hash (a
+//      shared table of positions from earlier rounds, updated with atomicMax after each round's lookups) and distances
+//      1..PB_GZ_SHORT (runs inside a round), every candidate verified byte by byte, the longest kept (the nearest on ties);
+//   3. walks the greedy parse through the round's matches on one thread, carrying the cursor into the next round, and
+//      appends the tokens to the block's token buffer (global scratch);
+//   4. counts the symbols with shared atomics and builds the code lengths on one thread (gz_code_lengths);
+//   5. writes a dynamic block -- header by one thread, then each thread's contiguous run of tokens at its scanned bit offset
+//      with atomicOr into zeroed shared words (disjoint bits) -- or stored blocks when those are not larger.
+// Every choice depends on the input alone (the hash table keeps the largest position, atomics only add or OR disjoint
+// bits), so the bytes are the same run to run.  sizes[1 + b] = the member's bytes (sizes[0] = 0), for scan_offsets.
+constexpr int PB_GZ_THREADS = 256;
+constexpr int PB_GZ_HASH_BITS = 12;
+constexpr int PB_GZ_SHORT = 8;
+constexpr int PB_GZ_WINDOW = 32768;
+constexpr int PB_GZ_MIN_BLOCK = 4096, PB_GZ_MAX_BLOCK = 131072, PB_GZ_DEFAULT_BLOCK = 65536;
+
+struct GzShared {                       // after the staged block and the hash table
+    uint32_t crc_tab[256];
+    uint32_t part[PB_GZ_THREADS];
+    uint16_t mlen[PB_GZ_THREADS], mdist[PB_GZ_THREADS];
+    uint32_t ll_freq[GZ_LITLEN], d_freq[GZ_DIST];
+    uint32_t work[2 * GZ_LITLEN + 16];
+    uint16_t ll_code[GZ_LITLEN], d_code[GZ_DIST];
+    uint8_t ll_len[GZ_LITLEN], d_len[GZ_DIST], all_lens[GZ_LITLEN + GZ_DIST];
+    GzDynHeader H;
+    unsigned long long body_bits, head_bits;
+    int32_t n_tok, stored;
+};
+__host__ __device__ __forceinline__ int64_t gz_stage_bytes(int32_t block) { return ((int64_t)block + 15) & ~(int64_t)15; }
+__host__ __device__ __forceinline__ int64_t gz_smem_bytes(int32_t block) {
+    return gz_stage_bytes(block) + 8 * (1 << PB_GZ_HASH_BITS) + (int64_t)sizeof(GzShared);
+}
+__device__ __forceinline__ uint32_t gz_hash(const uint8_t *p) {
+    return (((uint32_t)p[0] << 16) | ((uint32_t)p[1] << 8) | p[2]) * 2654435761u >> (32 - PB_GZ_HASH_BITS);
+}
+__device__ __forceinline__ int gz_match(const uint8_t *in, int p, int d, int maxl) {
+    int l = 0;
+    while (l < maxl && in[p + l - d] == in[p + l]) ++l;
+    return l;
+}
+// a token: bit 31 clear = literal byte; set = match, length - 3 in bits 16..23, distance - 1 in bits 0..14
+__device__ __forceinline__ int gz_token_bits(uint32_t tk, const GzShared &S) {
+    if (!(tk >> 31)) return S.ll_len[tk];
+    int ls, le, lv, ds, de, dv;
+    gz_len_sym((int)((tk >> 16) & 255u) + 3, ls, le, lv);
+    gz_dist_sym((int)(tk & 32767u) + 1, ds, de, dv);
+    return S.ll_len[ls] + le + S.d_len[ds] + de;
+}
+__device__ __forceinline__ void gz_or_bits(uint32_t *w, unsigned long long pos, uint32_t bits, int n) {
+    if (!n) return;
+    const int sh = (int)(pos & 31);
+    atomicOr(reinterpret_cast<int *>(w + (pos >> 5)), (int)(bits << sh));
+    if (sh + n > 32) atomicOr(reinterpret_cast<int *>(w + (pos >> 5) + 1), (int)(bits >> (32 - sh)));
+}
+__global__ void __launch_bounds__(PB_GZ_THREADS) gzip_block_kernel(const uint8_t *src, const int64_t *blk_start, const int64_t *blk_len,
+                                                                   int32_t block, uint8_t *slots, int64_t slot_stride,
+                                                                   uint32_t *tokens, int64_t *sizes) {
+    extern __shared__ uint32_t smem[];
+    const int t = threadIdx.x;
+    const int64_t b = blockIdx.x;
+    const int n = (int)blk_len[b];
+    const uint8_t *g = src + blk_start[b];
+    uint8_t *in = reinterpret_cast<uint8_t *>(smem);
+    unsigned long long *head = reinterpret_cast<unsigned long long *>(in + gz_stage_bytes(block));
+    GzShared &S = *reinterpret_cast<GzShared *>(in + gz_stage_bytes(block) + 8 * (1 << PB_GZ_HASH_BITS));
+    uint32_t *tok = tokens + b * (int64_t)block;
+    uint8_t *out = slots + b * slot_stride;
+
+    for (int i = t; i < n; i += PB_GZ_THREADS) in[i] = g[i];
+    for (int i = t; i < (1 << PB_GZ_HASH_BITS); i += PB_GZ_THREADS) head[i] = 0ull;
+    S.crc_tab[t] = gz_crc_table_entry((uint32_t)t);
+    for (int i = t; i < GZ_LITLEN + GZ_DIST; i += PB_GZ_THREADS) (i < GZ_LITLEN ? S.ll_freq[i] : S.d_freq[i - GZ_LITLEN]) = 0u;
+    __syncthreads();
+
+    // ---- 1. CRC-32 ----
+    const int per = (n + PB_GZ_THREADS - 1) / PB_GZ_THREADS;
+    {
+        const int lo = min(n, t * per), hi = min(n, lo + per);
+        S.part[t] = gz_crc_update(0u, S.crc_tab, in + lo, hi - lo);
+        for (int s = 1; s < PB_GZ_THREADS; s <<= 1) {
+            __syncthreads();
+            if ((t & (2 * s - 1)) == 0) {
+                const int r0 = min(n, (t + s) * per), r1 = min(n, (t + 2 * s) * per);
+                S.part[t] = gz_crc_combine(S.part[t], S.part[t + s], r1 - r0);
+            }
+        }
+    }
+    // ---- 2./3. matches in rounds, greedy parse ----
+    int cursor = 0, n_tok = 0;                            // thread 0's
+    for (int base = 0; base < n; base += PB_GZ_THREADS) {
+        const int p = base + t;
+        int best_len = 0, best_dist = 0;
+        if (p + 3 <= n) {
+            const int maxl = min(258, n - p);
+            for (int d = 1; d <= PB_GZ_SHORT && d <= p && best_len < maxl; ++d) {
+                const int l = gz_match(in, p, d, maxl);
+                if (l > best_len) { best_len = l; best_dist = d; }
+            }
+            const unsigned long long c = head[gz_hash(in + p)];
+            if (best_len < maxl && c) {
+                const int d = p - (int)(c - 1ull);
+                if (d > PB_GZ_SHORT && d <= PB_GZ_WINDOW) {
+                    const int l = gz_match(in, p, d, maxl);
+                    if (l > best_len) { best_len = l; best_dist = d; }
+                }
+            }
+        }
+        S.mlen[t] = (uint16_t)(best_len >= 3 ? best_len : 0);
+        S.mdist[t] = (uint16_t)best_dist;
+        __syncthreads();
+        if (p + 3 <= n) atomicMax(&head[gz_hash(in + p)], (unsigned long long)(p + 1));
+        if (t == 0) {
+            const int end = min(n, base + PB_GZ_THREADS);
+            while (cursor < end) {
+                const int l = S.mlen[cursor - base];
+                if (l) {
+                    tok[n_tok++] = 0x80000000u | ((uint32_t)(l - 3) << 16) | (uint32_t)(S.mdist[cursor - base] - 1);
+                    cursor += l;
+                } else {
+                    tok[n_tok++] = in[cursor++];
+                }
+            }
+            S.n_tok = n_tok;
+        }
+        __syncthreads();
+    }
+    const uint32_t crc = S.part[0];
+    // ---- 4. symbol counts, code lengths, the cheaper encoding ----
+    const int nt = S.n_tok;
+    for (int i = t; i < nt; i += PB_GZ_THREADS) {
+        const uint32_t tk = tok[i];
+        if (tk >> 31) {
+            int ls, le, lv, ds, de, dv;
+            gz_len_sym((int)((tk >> 16) & 255u) + 3, ls, le, lv);
+            gz_dist_sym((int)(tk & 32767u) + 1, ds, de, dv);
+            atomicAdd(&S.ll_freq[ls], 1u);
+            atomicAdd(&S.d_freq[ds], 1u);
+        } else {
+            atomicAdd(&S.ll_freq[tk], 1u);
+        }
+    }
+    __syncthreads();
+    if (t == 0) {
+        S.ll_freq[256] = 1u;                              // end of block
+        gz_code_lengths(S.ll_freq, GZ_LITLEN, GZ_MAX_BITS, S.ll_len, S.work);
+        gz_code_lengths(S.d_freq, GZ_DIST, GZ_MAX_BITS, S.d_len, S.work);
+        gz_canonical_codes(S.ll_len, GZ_LITLEN, S.ll_code);
+        gz_canonical_codes(S.d_len, GZ_DIST, S.d_code);
+        const unsigned long long head_bits = gz_dynamic_header(S.ll_len, S.d_len, S.H, S.all_lens, S.work);
+        unsigned long long body = 0;
+        for (int s = 0; s < GZ_LITLEN; ++s) body += (unsigned long long)S.ll_freq[s] * (S.ll_len[s] + gz_len_extra_bits(s));
+        for (int s = 0; s < GZ_DIST; ++s) body += (unsigned long long)S.d_freq[s] * (S.d_len[s] + gz_dist_extra_bits(s));
+        S.head_bits = head_bits;
+        S.body_bits = body;
+        S.stored = (int64_t)((head_bits + body + 7) / 8) >= gz_stored_bytes(n);
+    }
+    __syncthreads();
+    // ---- 5. the member ----
+    int64_t bytes;
+    if (S.stored) {
+        const int nst = (n + GZ_STORED_MAX - 1) / GZ_STORED_MAX;
+        for (int i = t; i < n; i += PB_GZ_THREADS) out[GZ_HEADER + 5 * (i / GZ_STORED_MAX + 1) + i] = in[i];
+        for (int k = t; k < nst; k += PB_GZ_THREADS) {
+            uint8_t *h = out + GZ_HEADER + (int64_t)k * (GZ_STORED_MAX + 5);
+            const int len = min(GZ_STORED_MAX, n - k * GZ_STORED_MAX);
+            h[0] = (uint8_t)(k == nst - 1);
+            h[1] = (uint8_t)len; h[2] = (uint8_t)(len >> 8);
+            h[3] = (uint8_t)~len; h[4] = (uint8_t)(~len >> 8);
+        }
+        bytes = GZ_HEADER + gz_stored_bytes(n) + GZ_TRAILER;
+    } else {
+        // the deflate bits go to zeroed shared words over the staged block and the hash table, which are no longer needed
+        const unsigned long long total = 8ull * GZ_HEADER + S.head_bits + S.body_bits;
+        bytes = (int64_t)((total + 7) / 8) + GZ_TRAILER;
+        uint32_t *w = smem;
+        for (int i = t; i < (int)((bytes + 3) / 4); i += PB_GZ_THREADS) w[i] = 0u;
+        __syncthreads();
+        if (t == 0) {
+            GzBitWriter bw{w, 0};
+            const uint8_t hdr[GZ_HEADER] = {0x1f, 0x8b, 8, 0, 0, 0, 0, 0, 0, 3};
+            for (int i = 0; i < GZ_HEADER; ++i) bw.put(hdr[i], 8);
+            gz_write_dynamic_header(bw, 1, S.H);
+        }
+        __syncthreads();
+        const int tper = (nt + PB_GZ_THREADS - 1) / PB_GZ_THREADS;
+        const int t0 = min(nt, t * tper), t1 = min(nt, t0 + tper);
+        long long mine = 0, all = 0;
+        for (int i = t0; i < t1; ++i) mine += gz_token_bits(tok[i], S);
+        unsigned long long pos = 8ull * GZ_HEADER + S.head_bits + (unsigned long long)block_exclusive_scan(mine, &all);
+        for (int i = t0; i < t1; ++i) {
+            const uint32_t tk = tok[i];
+            if (!(tk >> 31)) {
+                gz_or_bits(w, pos, S.ll_code[tk], S.ll_len[tk]);
+                pos += S.ll_len[tk];
+                continue;
+            }
+            int ls, le, lv, ds, de, dv;
+            gz_len_sym((int)((tk >> 16) & 255u) + 3, ls, le, lv);
+            gz_dist_sym((int)(tk & 32767u) + 1, ds, de, dv);
+            gz_or_bits(w, pos, S.ll_code[ls], S.ll_len[ls]);
+            pos += S.ll_len[ls];
+            gz_or_bits(w, pos, (uint32_t)lv, le);
+            pos += le;
+            gz_or_bits(w, pos, S.d_code[ds], S.d_len[ds]);
+            pos += S.d_len[ds];
+            gz_or_bits(w, pos, (uint32_t)dv, de);
+            pos += de;
+        }
+        __syncthreads();
+        if (t == 0) {                                     // end of block; the trailer starts at the next byte
+            GzBitWriter bw{w, 8ull * GZ_HEADER + S.head_bits + (unsigned long long)all};
+            bw.put(S.ll_code[256], S.ll_len[256]);
+        }
+        __syncthreads();
+        const uint8_t *wb = reinterpret_cast<const uint8_t *>(w);
+        for (int64_t i = t; i < bytes - GZ_TRAILER; i += PB_GZ_THREADS) out[i] = wb[i];
+    }
+    if (S.stored && t < GZ_HEADER) {
+        const uint8_t hdr[GZ_HEADER] = {0x1f, 0x8b, 8, 0, 0, 0, 0, 0, 0, 3};
+        out[t] = hdr[t];
+    }
+    if (t < GZ_TRAILER) out[bytes - GZ_TRAILER + t] = (uint8_t)((t < 4 ? crc : (uint32_t)n) >> (8 * (t & 3)));
+    if (t == 0) {
+        sizes[1 + b] = bytes;
+        if (b == 0) sizes[0] = 0;
+    }
+}
+
+// ---------------------------------------------------------------------------------------------------
 // generic_kernel: int32, one thread per alignment, column sweep with S/Hs columns and a byte trace in
 // global scratch.  Only used for inputs outside the int16 domain (huge scores, positive gap scores,
 // adapters longer than 256) -- slow but exact for every scoring scheme the C-ABI accepts.

@@ -29,6 +29,14 @@ grouped by bin, so that each bin's reads are one contiguous slice of records and
     for name, (b0, b1) in em.bins.items():           # the bytes demux_fastq writes into <name>.fastq
         open(name + '.fastq', 'wb').write(data[b0:b1].numpy())
 
+gzip_bytes (pb200GzipDevice) compresses such bytes on the device -- one gzip file per bin, each a run of independent members
+-- so that a `.gz` output also comes home in one copy, smaller by the compression ratio:
+
+    gz = device_reads.gzip_bytes(em.data, em.bins)   # em.bins: None for one file
+    data = torch.empty(gz.data.numel(), dtype=torch.uint8, pin_memory=True).copy_(gz.data)
+    for name, (b0, b1) in gz.ranges.items():
+        open(name + '.fastq.gz', 'wb').write(data[b0:b1].numpy())
+
 The device work runs on torch.cuda.current_stream(); the call returns when the outputs are written.  `W` (the engine's
 wrapper module) and `device()` (the allocator) are module attributes, so that the same set handling and retry logic can run
 on another engine build.
@@ -43,6 +51,7 @@ from . import fastq
 TrimmedReads = collections.namedtuple('TrimmedReads', 'seq qual off read part start_trim end_trim hits calls')
 DemuxedReads = collections.namedtuple('DemuxedReads', 'seq qual off read part bins calls start_trim end_trim hits')
 EmittedReads = collections.namedtuple('EmittedReads', 'data off bins')
+GzippedBytes = collections.namedtuple('GzippedBytes', 'data ranges')
 
 
 class TorchDevice:
@@ -303,6 +312,36 @@ def emit_reads(out, names, name_off, rna=None, fmt='fastq'):
     return EmittedReads(D.head(data, n_out), off, bins)
 
 
+def gzip_bytes(data, ranges=None, block=0):
+    """gzip on the device (pb200GzipDevice): data is a contiguous 1-D uint8 CUDA tensor (e.g. emit_reads(...).data); ranges =
+    {name: (first byte, end byte)} of files inside it (e.g. EmittedReads.bins; non-overlapping), or None for one file.  Every
+    file is compressed on its own as a run of gzip members of `block` input bytes (0 = the engine's default), so that each
+    file's compressed bytes are one slice of the result.  Bytes outside every range are compressed too but belong to no name.
+    Returns GzippedBytes: data (uint8 on the device, exactly the compressed length) and ranges = {name: (first byte, end
+    byte)} in it (None when ranges is None)."""
+    D = device()
+    if hasattr(D, 'check_bytes'):
+        D.check_bytes(data)
+    n = D.numel(data)
+    spans = sorted(((int(b0), int(b1), name) for name, (b0, b1) in (ranges or {}).items()), key=lambda x: x[:2])
+    cuts, seg_of, at = [0], {}, 0
+    for b0, b1, name in spans:
+        if b0 < at or b1 < b0 or b1 > n:
+            raise ValueError('ranges must be non-overlapping (first, end) byte ranges inside data')
+        if b0 > at:
+            cuts.append(b0)
+        seg_of[name] = len(cuts) - 1
+        cuts.append(b1)
+        at = b1
+    if at < n or len(cuts) == 1:
+        cuts.append(n)
+    cap = W.gzip_bound(n, len(cuts) - 1, block)
+    out = D.empty(max(cap, 1), np.uint8)
+    total, off = W.pb200_gzip_device(D.ptr(data), n, cuts, block=block, d_out_ptr=D.ptr(out), out_cap=cap, stream_ptr=D.stream())
+    return GzippedBytes(D.head(out, total),
+                        None if ranges is None else {name: (int(off[k]), int(off[k + 1])) for name, k in seg_of.items()})
+
+
 # ---- bytes in: FASTQ / FASTA parsed on the device, and whole chunks from input bytes to output bytes ------------------------
 ParsedReads = collections.namedtuple('ParsedReads', 'names name_off seq seq_off qual rna kind')
 
@@ -391,9 +430,10 @@ def _host_batch(data, kind):
     return fastq.parse_fasta(data) if kind == 'fasta' else fastq.parse_fastq(data)
 
 
-def _device_chunk(data, kind, matching_sets, fmt, end_threshold, run):
-    """upload -> parse_reads -> run(parsed) -> emit_reads; None when the host path must take this chunk (a quality line longer
-    than its bases, no reads, nothing to align, or inputs the device call does not take: PB200_ERR_ARG)"""
+def _device_chunk(data, kind, matching_sets, fmt, end_threshold, run, gz=False):
+    """upload -> parse_reads -> run(parsed) -> emit_reads (-> gzip_bytes with gz) -> one copy home: (records, the bins' byte
+    ranges in the copy or None, the copy, reads); None when the host path must take this chunk (a quality line longer than its
+    bases, no reads, nothing to align, or inputs the device call does not take: PB200_ERR_ARG)"""
     if fmt not in ('fastq', 'fasta'):
         raise ValueError("fmt must be 'fastq' or 'fasta'")
     sets = fastq._norm_sets(matching_sets)
@@ -415,26 +455,46 @@ def _device_chunk(data, kind, matching_sets, fmt, end_threshold, run):
             raise
         return None
     em = emit_reads(out, p.names, p.name_off, p.rna, fmt)
-    return out, em, getattr(D, 'download', D.host)(em.data), n
+    data, bins = (em.data, em.bins) if not gz else gzip_bytes(em.data, em.bins)
+    return out, bins, getattr(D, 'download', D.host)(data), n
+
+
+def _gzip_host_output(parts):
+    """the host path's output (bytes, or {bin: bytes}) compressed by gzip_bytes like a device chunk's: (copy home, ranges)"""
+    D = device()
+    named = parts if isinstance(parts, dict) else {None: parts}
+    ranges, at = {}, 0
+    for name, b in named.items():
+        ranges[name] = (at, at + len(b))
+        at += len(b)
+    flat = b''.join(bytes(b) for b in named.values())
+    g = gzip_bytes(_upload(D, np.frombuffer(flat, dtype=np.uint8)), ranges)
+    return getattr(D, 'download', D.host)(g.data), g.ranges
 
 
 def trim_fastq(data, matching_sets, scoring_scheme_vals, end_size=150, extra_end_trim=2, end_threshold=75.0, min_trim_size=4,
                no_split=False, middle_threshold=85.0, extra_middle_trim_good_side=10, extra_middle_trim_bad_side=100,
-               min_split_read_size=1000, discard_middle=False, fmt='fastq', as_array=False, kind=None):
+               min_split_read_size=1000, discard_middle=False, fmt='fastq', as_array=False, kind=None, gz=False):
     """fastq.trim_fastq on the device from input bytes to output bytes: host bytes of whole FASTQ / FASTA records (kind: 'fastq',
     'fasta' or None = from the first byte) go up once, parse_reads -> trim_reads -> emit_reads run in GPU memory, and the output
     bytes come home in one copy.  Returns (output bytes, or a uint8 array with as_array; info with start_trim, end_trim and
     n_reads) -- the bytes fastq.trim_fastq writes for the parsed reads.  A chunk the device path does not take (a quality line
     longer than its bases, inputs adapterTrimSplitReadsDevice refuses) runs through fastq.trim_fastq instead, with the same
-    result.  Malformed input raises the host parser's ValueError."""
+    result.  Malformed input raises the host parser's ValueError.  gz=True: the output bytes are gzip members (gzip_bytes),
+    compressed on the device before the copy home; a chunk the host path takes is uploaded and compressed the same way."""
     opts = dict(end_size=end_size, extra_end_trim=extra_end_trim, end_threshold=end_threshold, min_trim_size=min_trim_size,
                 no_split=no_split, middle_threshold=middle_threshold, extra_middle_trim_good_side=extra_middle_trim_good_side,
                 extra_middle_trim_bad_side=extra_middle_trim_bad_side, min_split_read_size=min_split_read_size,
                 discard_middle=discard_middle)
     got = _device_chunk(data, kind, matching_sets, fmt, end_threshold,
-                        lambda p, n: trim_reads(p.seq, p.seq_off, matching_sets, scoring_scheme_vals, p.qual, **opts))
+                        lambda p, n: trim_reads(p.seq, p.seq_off, matching_sets, scoring_scheme_vals, p.qual, **opts), gz)
     if got is None:
-        return fastq.trim_fastq(_host_batch(data, kind), matching_sets, scoring_scheme_vals, fmt=fmt, as_array=as_array, **opts)
+        res, info = fastq.trim_fastq(_host_batch(data, kind), matching_sets, scoring_scheme_vals, fmt=fmt,
+                                     as_array=as_array and not gz, **opts)
+        if not gz:
+            return res, info
+        host, _ = _gzip_host_output(res)
+        return (host if as_array else host.tobytes()), info
     out, _, host, n = got
     info = {'start_trim': np.asarray(out.start_trim, dtype=np.int64), 'end_trim': np.asarray(out.end_trim, dtype=np.int64),
             'hits': out.hits, 'n_reads': n}
@@ -445,11 +505,12 @@ def demux_fastq(data, matching_sets, scoring_scheme_vals, forward_or_reverse='fo
                 end_threshold=75.0, min_trim_size=4, no_split=False, middle_threshold=85.0, extra_middle_trim_good_side=10,
                 extra_middle_trim_bad_side=100, min_split_read_size=1000, discard_middle=False, barcode_threshold=75.0,
                 barcode_diff=5.0, require_two_barcodes=False, discard_unassigned=False, untrimmed=False, fmt='fastq',
-                albacore_calls=None, as_array=False, kind=None):
+                albacore_calls=None, as_array=False, kind=None, gz=False):
     """fastq.demux_fastq on the device from input bytes to output bytes, as trim_fastq: parse_reads -> demux_reads -> emit_reads,
     and every bin's bytes are one slice of the single copy home.  albacore_calls: one bin name (or None) per read, one name for
     every read, or None.  Returns ({bin name: bytes (or uint8 arrays with as_array)}, info with calls, start_trim, end_trim and
-    n_reads); chunks the device path does not take run through fastq.demux_fastq, with the same result."""
+    n_reads); chunks the device path does not take run through fastq.demux_fastq, with the same result.  gz=True: every bin's
+    bytes are gzip members, compressed on the device as in trim_fastq."""
     opts = dict(end_size=end_size, extra_end_trim=extra_end_trim, end_threshold=end_threshold, min_trim_size=min_trim_size,
                 no_split=no_split, middle_threshold=middle_threshold, extra_middle_trim_good_side=extra_middle_trim_good_side,
                 extra_middle_trim_bad_side=extra_middle_trim_bad_side, min_split_read_size=min_split_read_size,
@@ -461,13 +522,17 @@ def demux_fastq(data, matching_sets, scoring_scheme_vals, forward_or_reverse='fo
         return [albacore_calls] * n if isinstance(albacore_calls, str) else albacore_calls
     got = _device_chunk(data, kind, matching_sets, fmt, end_threshold,
                         lambda p, n: demux_reads(p.seq, p.seq_off, matching_sets, scoring_scheme_vals, p.qual,
-                                                 albacore_calls=calls_for(n), **bc, **opts))
+                                                 albacore_calls=calls_for(n), **bc, **opts), gz)
     if got is None:
         batch = _host_batch(data, kind)
-        return fastq.demux_fastq(batch, matching_sets, scoring_scheme_vals, fmt=fmt, albacore_calls=calls_for(len(batch)),
-                                 as_array=as_array, **bc, **opts)
-    out, em, host, n = got
-    bins = {name: host[b0:b1] if as_array else host[b0:b1].tobytes() for name, (b0, b1) in em.bins.items()}
+        res, info = fastq.demux_fastq(batch, matching_sets, scoring_scheme_vals, fmt=fmt, albacore_calls=calls_for(len(batch)),
+                                      as_array=as_array and not gz, **bc, **opts)
+        if not gz:
+            return res, info
+        host, ranges = _gzip_host_output(res)
+        return {name: host[b0:b1] if as_array else host[b0:b1].tobytes() for name, (b0, b1) in ranges.items()}, info
+    out, ranges, host, n = got
+    bins = {name: host[b0:b1] if as_array else host[b0:b1].tobytes() for name, (b0, b1) in ranges.items()}
     info = {'start_trim': np.asarray(out.start_trim, dtype=np.int64), 'end_trim': np.asarray(out.end_trim, dtype=np.int64),
             'hits': out.hits, 'calls': out.calls, 'n_reads': n}
     return bins, info

@@ -22,7 +22,10 @@ PB200_DEVICE_DECISIONS=1 and PB200_DEVICE_MIDDLE=1 both set, each chunk's Phase 
 PB200_DEVICE_READS=1 takes each chunk from input bytes to output bytes on the device (device_reads.trim_fastq /
 demux_fastq): the raw bytes go up, are parsed there (pb200ParseReadsDevice), trimmed, split or demultiplexed and formatted
 there, and the output bytes come home in one copy; the background thread only reads (and gunzips) the input.  Chunks with
-nothing to align (no adapter set matched) and Phase A keep the host parse.
+nothing to align (no adapter set matched) and Phase A keep the host parse.  With PB200_DEVICE_READS=1, PB200_DEVICE_GZIP=1
+also compresses a .gz output on the device (device_reads.gzip_bytes: 64 KiB gzip members, a ratio between zlib's levels 1
+and 6 is not promised) before the one copy home; chunks with nothing to align are still compressed by the host.  It is a
+trade of compression ratio against time, like PB200_GZIP_LEVEL, so it stays the user's choice.
 
 Multi-GPU: launched with torchrun (one process per GPU) chunk c is handled by rank c % world on its own device; ranks
 write self-contained pieces and rank 0 stitches them in chunk order after a barrier -- no data-path collective
@@ -109,12 +112,13 @@ class _Sink:
         self.path = path if not self.ranked else '%s.rank%d' % (path, rank)
         self.index = []                                    # ranked mode: [chunk, offset, length]
 
-    def write(self, payload, chunk=0):
+    def write(self, payload, chunk=0, packed=False):
+        """packed: payload is already gzip members (compressed on the device) and is written as it is"""
         if not len(payload):
             return
         if self.f is None:
             self.f = sys.stdout.buffer if self.final is None else open(self.path, 'wb')
-        if self.gz:
+        if self.gz and not packed:
             level = int(os.environ.get('PB200_GZIP_LEVEL', 6))
             packed = hostio.gzip_members(payload, level)
             payload = packed if packed is not None else gzip.compress(bytes(payload), level)
@@ -179,6 +183,7 @@ def main():
     device_reads = None
     if os.environ.get('PB200_DEVICE_READS', '0') == '1':
         from . import device_reads
+    device_gzip = device_reads is not None and os.environ.get('PB200_DEVICE_GZIP', '0') == '1'
     if world > 1:
         import torch.distributed as dist
         from . import cpp_function_wrappers as W
@@ -271,16 +276,17 @@ def main():
     def process(batch, albacore_call, chunk):
         # batch: a FastqBatch, or with PB200_DEVICE_READS=1 (kind, raw bytes) -- parsed on the host only when nothing is aligned
         on_device = device_reads is not None and sets
+        packed = bool(on_device and gz and device_gzip)      # the device path's bytes come home compressed
         if device_reads is not None and not sets:
             batch = parsers[batch[0]](batch[1])
         if args.barcode_dir is None:
             if on_device:
-                out, _ = device_reads.trim_fastq(batch[1], sets, scoring, kind=batch[0], **common)
+                out, _ = device_reads.trim_fastq(batch[1], sets, scoring, kind=batch[0], gz=packed, **common)
             elif sets:
                 out, _ = fastq.trim_fastq(batch, sets, scoring, **common)
             else:                   # "No adapters found - output reads are unchanged from input reads"
                 out = fastq.emit(batch, fmt=fmt, as_array=True)
-            sink(None).write(out, chunk)
+            sink(None).write(out, chunk, packed)
             return
         if sets:
             bc = dict(barcode_threshold=args.barcode_threshold, barcode_diff=args.barcode_diff,
@@ -288,7 +294,7 @@ def main():
                       untrimmed=args.untrimmed)
             if on_device:
                 bins, _ = device_reads.demux_fastq(batch[1], sets, scoring, direction, albacore_calls=albacore_call,
-                                                   kind=batch[0], **bc, **common)
+                                                   kind=batch[0], gz=packed, **bc, **common)
             else:
                 calls = None if albacore_call is None else [albacore_call] * len(batch)
                 bins, _ = fastq.demux_fastq(batch, sets, scoring, direction, albacore_calls=calls, **bc, **common)
@@ -296,7 +302,7 @@ def main():
             out = fastq.emit(batch, fmt=fmt, untrimmed=args.untrimmed, as_array=True)
             bins = {} if args.discard_unassigned else {'none': out}
         for name, payload in bins.items():
-            sink(name).write(payload, chunk)
+            sink(name).write(payload, chunk, packed)
 
     def batches():
         chunk = 0

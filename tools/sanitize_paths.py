@@ -173,5 +173,24 @@ def demux_reads():
 
 
 run('demux_dev', {}, demux_reads)
+
+
+# gzip members written on the device (pb200GzipDevice): small inputs in several segments, decompressed bin by bin
+def gzip_members():
+    import gzip
+    import torch
+    from porechop_b200 import device_reads
+    rng = np.random.default_rng(5)
+    data = b''.join(b'@r%d\n' % k + rng.integers(65, 69, 300 + 97 * k, dtype=np.uint8).tobytes() + b'\n+\n' +
+                    bytes(330 + 97 * k - 30) + b'\n' for k in range(12))
+    cuts = [0, 0, 5, 4096, 4097, 9000, len(data)]
+    ranges = {'s%d' % k: (cuts[k], cuts[k + 1]) for k in range(len(cuts) - 1)}
+    g = device_reads.gzip_bytes(torch.from_numpy(np.frombuffer(data, dtype=np.uint8).copy()).cuda(), ranges, block=4096)
+    host = g.data.cpu().numpy().tobytes()
+    got = b''.join(gzip.decompress(host[b0:b1]) for b0, b1 in g.ranges.values())
+    return np.frombuffer(got, dtype=np.uint8), np.frombuffer(data, dtype=np.uint8)
+
+
+run('gzip_dev', {}, gzip_members)
 print('SANITIZE RUN COMPLETE, %d wrong' % bad, flush=True)
 sys.exit(1 if bad else 0)
